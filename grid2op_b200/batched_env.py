@@ -28,6 +28,7 @@ The topology lives on the HOST (int8 [batch, n_topo_in]); a step that changed it
 """
 from __future__ import annotations
 
+import os
 from typing import Optional
 
 import numpy as np
@@ -103,6 +104,10 @@ class BatchedEnv(BatchedDoNothing):
         self.nb_cap = self._bus_cap() if self.tight_cap else 0
         self.n_illegal = 0
         self.n_steps = 0
+        self.is_illegal = np.zeros(B, dtype=bool)                          # the last step's action was replaced by "do nothing"
+        self.current_step = np.zeros(B, dtype=np.int32)                    # env.nb_time_step (obs.current_step)
+        self.soft_overflow_threshold = float(kw.get("soft_overflow_threshold", 1.0))
+        self._obs = None
 
     # ------------------------------------------------------------------------------------------------------------
     def _bus_cap(self) -> int:
@@ -182,6 +187,7 @@ class BatchedEnv(BatchedDoNothing):
         if has_line.any():
             illegal |= has_line & (self.line_cooldown[idx, np.where(has_line, line_id, 0)] > 0)
         self.n_illegal += int((illegal & ~self.done).sum())
+        self.is_illegal = illegal & ~self.done
         ok = ~illegal & ~self.done
         if has_sub.any():
             keep = ok[who_s]
@@ -312,7 +318,15 @@ class BatchedEnv(BatchedDoNothing):
         self.done |= newly_done
         self.row = self.row + 1
         self.n_steps += 1
-        return rho, self.done.copy(), {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done}
+        if from_reset:
+            self.is_illegal = np.zeros(self.batch, dtype=bool)
+            self.current_step[live] = 0
+            if self._obs is not None:
+                self._obs["reset"][live] = True
+        else:
+            self.current_step[live] += 1
+        return rho, self.done.copy(), {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done,
+                                       "is_illegal": self.is_illegal.copy()}
 
     def line_angles(self, out: np.ndarray):
         """``theta_or, theta_ex`` [B, n_line] of the full result records ``out`` (:meth:`fetch`) as an OBSERVATION of the reference
@@ -356,11 +370,88 @@ class BatchedEnv(BatchedDoNothing):
         self.last_bus[idx] = np.where(self.topo0[idx, :self.gm.dim_topo] > 0, self.topo0[idx, :self.gm.dim_topo], 1)
         self.line_cooldown[idx] = 0; self.sub_cooldown[idx] = 0
         self.done[idx] = False
+        self.current_step[idx] = 0; self.is_illegal[idx] = False
+        if self._obs is not None:
+            self._obs["reset"][idx] = True
         self.row[idx] = rows
         self.engine.series_reset_instances(idx, t_new=rows % self.chron.shape[1], topo_rows=self.topo[idx])
         self._cap_dirty[idx] = True
         if self.tight_cap:
             self.nb_cap = self._bus_cap()
+
+    # ---- observation layer ---------------------------------------------------------------------------------------------
+    def enable_observation(self, env_dir: str, attrs=None, reward: Optional[str] = "RedispReward", scenarios=None,
+                           init_storage_capacity: float = 0.5, activate_storage_loss: bool = True):
+        """Let :meth:`observe` assemble grid2op observation vectors (``obs.to_vect()`` of the attribute list ``attrs``, default
+        ``CompleteObservation.attr_list_vect``; pass the environment's own observation class list or a gym-style subset) and
+        rewards (``"RedispReward"``, ``"L2RPNReward"`` or None) on the device.  ``env_dir``: the environment folder
+        (``prods_charac.csv``, ``storage_units_charac.csv``, ``chronics/``); ``scenarios``: the chronics folders in the order of
+        the ``chron`` array (default: every folder of ``env_dir/chronics``, sorted, as :func:`chronics.load_scenarios` reads them)."""
+        from . import observation as ob
+        from .chronics import list_scenarios
+        if reward not in ob.REWARDS:
+            raise ValueError(f"unknown reward class {reward!r} (RedispReward, L2RPNReward or None)")
+        gm = self.gm
+        seg, n_obs = ob.obs_spec(gm, attrs)
+        folders = list(scenarios) if scenarios is not None else list_scenarios(os.path.join(env_dir, "chronics"))
+        if len(folders) != self.chron.shape[0]:
+            raise ValueError(f"{len(folders)} scenario folders for {self.chron.shape[0]} scenarios of the chronics array")
+        cal, dt_min, max_step = ob.load_calendar(folders, self.chron.shape[1])
+        gen = ob.load_gen_charac(env_dir, gm)
+        if reward == "RedispReward" and not gen["available"]:
+            raise ValueError("RedispReward needs the generator costs of prods_charac.csv")
+        t = dict(seg=seg, n_obs=n_obs, calendar=cal, max_step=max_step, delta_time=dt_min, gen=gen,
+                 storage=ob.load_storage(env_dir, gm, dt_min, init_storage_capacity, activate_storage_loss),
+                 maint_time=self._maint_time, maint_dur=self._maint_dur, reward_kind=ob.REWARDS[reward],
+                 reward=ob.reward_constants(gen, dt_min) if gen["available"] else dict(max_regret=0.0, reward_min=0.0, reward_illegal=0.0,
+                                                                                       dts_hours=dt_min / 60.0),
+                 soft_thr=self.soft_overflow_threshold)
+        if reward == "L2RPNReward":
+            t["reward"]["reward_min"] = 0.0
+        self.engine.obs_bind(t)
+        self._obs = dict(tables=t, n_obs=n_obs, reward=reward, reset=np.ones(self.batch, dtype=bool),
+                         host_in=np.zeros((self.batch, gm.n_line + gm.n_sub + 3), dtype=np.int32))
+        return n_obs
+
+    def observe_inputs(self) -> np.ndarray:
+        """int32 [B, n_line + n_sub + 3]: the per-instance values only the host knows (cooldowns, current_step, step stamp, flags
+        illegal / game over / reset) — what one observe launch copies to the device."""
+        gm, o = self.gm, self._obs
+        h = o["host_in"]
+        nl, ns = gm.n_line, gm.n_sub
+        h[:, :nl] = self.line_cooldown; h[:, nl:nl + ns] = self.sub_cooldown
+        h[:, nl + ns] = self.current_step; h[:, nl + ns + 1] = self.n_steps
+        h[:, nl + ns + 2] = self.is_illegal * 1 + self.done * 2 + o["reset"] * 4
+        return h
+
+    def observe(self, obs_out=None, reward_out=None):
+        """grid2op observation vectors and rewards of the last step for the whole batch -> ``(obs [B, n_obs], reward [B])`` as torch
+        CUDA tensors (``obs_out`` / ``reward_out``: caller-owned float32 tensors to write into).  One launch on the engine's stream
+        behind the step; the result records never leave the device.  Call it once after every step: the overflow counters of the
+        vector advance with it.  With a host-side engine (tests) numpy arrays come back."""
+        if self._obs is None:
+            raise RuntimeError("call enable_observation() first")
+        B, n_obs = self.batch, self._obs["n_obs"]
+        host_in = self.observe_inputs()
+        if not hasattr(self.engine, "h"):                 # host-side engine (test infrastructure): numpy in / out
+            obs, rew = self.engine.observe_host(host_in, obs_out, reward_out)
+            self._obs["reset"][:] = False
+            return obs, rew
+        import torch
+        dev = torch.device("cuda", getattr(self.engine, "device", 0))
+        obs = obs_out if obs_out is not None else torch.empty((B, n_obs), dtype=torch.float32, device=dev)
+        rew = reward_out if reward_out is not None else torch.empty(B, dtype=torch.float32, device=dev)
+        if obs.dtype != torch.float32 or tuple(obs.shape) != (B, n_obs) or not obs.is_cuda or not obs.is_contiguous():
+            raise ValueError(f"obs_out must be a contiguous float32 CUDA tensor of shape {(B, n_obs)}")
+        if rew.dtype != torch.float32 or tuple(rew.shape) != (B,) or not rew.is_cuda or not rew.is_contiguous():
+            raise ValueError(f"reward_out must be a contiguous float32 CUDA tensor of shape {(B,)}")
+        cur = torch.cuda.current_stream(obs.device)
+        eng_stream = torch.cuda.ExternalStream(self.engine.stream, device=obs.device)
+        eng_stream.wait_stream(cur)                       # (the tensors may have been written on torch's stream)
+        self.engine.observe(host_in, obs.data_ptr(), rew.data_ptr())
+        cur.wait_stream(eng_stream)                       # torch's consumers run behind the observe launch (no host sync)
+        self._obs["reset"][:] = False
+        return obs, rew
 
     def reset_step(self):
         """the solve ``env.reset()`` performs on the first row (no soft-overflow counting, no cooldown from actions)"""

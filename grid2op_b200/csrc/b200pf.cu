@@ -6,6 +6,7 @@
 #include "b200pf_sparse.cuh"
 #include "b200pf_block.cuh"
 #include "b200pf_redo.cuh"
+#include "b200pf_obs.cuh"
 #include "../../include/b200pf.h"
 
 #include <cstdio>
@@ -103,6 +104,12 @@ struct b200pf_handle {
     bool on_side_stream = false;                            // a chunk / group launch is being issued (h->stream is swapped for it)
     cudaEvent_t inst_plan_ev = nullptr; bool inst_plan_pending = false;   // last H2D copy out of h_inst_plan
     int last_smem = 0, last_T = 0, last_grid = 0, last_block = 0;
+    // observation layer (b200pf_obs_bind / b200pf_observe)
+    ObsArgs obs{}; int obs_batch = 0, obs_rows = 0;
+    std::vector<void *> obs_allocs;
+    int32_t *h_obs_in = nullptr, *d_obs_in = nullptr;       // pinned host record of the per-instance inputs and its device copy
+    cudaEvent_t obs_ev = nullptr; bool obs_ev_pending = false;
+    int64_t obs_launches = 0, obs_h2d_bytes = 0, d2h_bytes = 0;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -297,6 +304,9 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     for (auto &cs : h->group_stream) if (cs) { cudaStreamSynchronize(cs); cudaStreamDestroy(cs); }
     for (auto &ev : h->group_event) if (ev) cudaEventDestroy(ev);
     if (h->inst_plan_ev) cudaEventDestroy(h->inst_plan_ev);
+    for (void *p : h->obs_allocs) cudaFree(p);
+    if (h->h_obs_in) cudaFreeHost(h->h_obs_in);
+    if (h->obs_ev) cudaEventDestroy(h->obs_ev);
     delete h;
     return 0;
 }
@@ -1323,6 +1333,7 @@ extern "C" int b200pf_series_fetch_state(b200pf_handle *h, int32_t *pc, int32_t 
     CU(cudaSetDevice(h->device));
     CU(cudaStreamSynchronize(h->stream));
     const size_t B = (size_t)h->series_batch, nl = (size_t)h->g.n_line;
+    h->d2h_bytes += (int64_t)(((pc != nullptr) + (tso != nullptr) + (disc != nullptr)) * B * nl * 4 + (done != nullptr) * B * 4);
     if (pc) CU(cudaMemcpy(pc, h->d_pcount, B * nl * 4, cudaMemcpyDeviceToHost));
     if (tso) CU(cudaMemcpy(tso, h->d_tsover, B * nl * 4, cudaMemcpyDeviceToHost));
     if (disc) CU(cudaMemcpy(disc, h->d_disc, B * nl * 4, cudaMemcpyDeviceToHost));
@@ -1347,6 +1358,7 @@ extern "C" int b200pf_series_fetch(b200pf_handle *h, float *out, int32_t *status
     const size_t B = (size_t)h->series_batch;
     const DevGrid &g = h->g;
     CU(cudaStreamSynchronize(h->stream));
+    h->d2h_bytes += (int64_t)((out != nullptr) * B * g.n_out * 4 + ((status != nullptr) + (iters != nullptr)) * B * 4 + (rho != nullptr) * B * g.n_line * 4);
     if (out) CU(cudaMemcpy(out, h->x_out ? h->x_out : h->d_out, B * g.n_out * 4, cudaMemcpyDeviceToHost));
     if (status) CU(cudaMemcpy(status, h->x_status ? h->x_status : h->d_status, B * 4, cudaMemcpyDeviceToHost));
     if (iters) CU(cudaMemcpy(iters, h->x_iters ? h->x_iters : h->d_iters, B * 4, cudaMemcpyDeviceToHost));
@@ -1647,6 +1659,106 @@ extern "C" int64_t b200pf_redo_launch_count(const b200pf_handle *h) { return h ?
 extern "C" int b200pf_plan_counters(const b200pf_handle *h, int64_t *out4) {
     if (!h || !out4) return fail(B200PF_E_ARG, "null pointer");
     out4[0] = h->plan_lookups; out4[1] = h->plan_hits; out4[2] = h->plans_built; out4[3] = h->plan_cache_resets;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// observation layer: grid2op observation vectors + rewards of the bound series, assembled on the device (b200pf_obs.cuh)
+// ------------------------------------------------------------------------------------------------
+extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
+    if (d->n_seg < 0 || d->n_obs < 0 || (d->n_seg && !d->seg) || !d->calendar || !d->max_step) return fail(B200PF_E_ARG, "bad observation spec");
+    const DevGrid &g = h->g;
+    if (g.n_gen && (!d->gen_pmin || !d->gen_pmax || !d->gen_ramp_up || !d->gen_ramp_down || !d->gen_cost || !d->gen_renewable))
+        return fail(B200PF_E_ARG, "generator tables missing");
+    if (g.n_sto && (!d->sto_charge0 || !d->sto_loss_step)) return fail(B200PF_E_ARG, "storage tables missing");
+    if (d->reward_kind < B200PF_REWARD_NONE || d->reward_kind > B200PF_REWARD_L2RPN) return fail(B200PF_E_ARG, "unknown reward kind");
+    for (int s = 0; s < d->n_seg; ++s)
+        if (d->seg[3 * s] < 0 || d->seg[3 * s] >= OS_N_SOURCES || d->seg[3 * s + 1] < 0 || d->seg[3 * s + 2] < 0 ||
+            d->seg[3 * s + 1] + d->seg[3 * s + 2] > d->n_obs) return fail(B200PF_E_ARG, "observation segment out of range");
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (void *p : h->obs_allocs) cudaFree(p);
+    h->obs_allocs.clear();
+    if (h->h_obs_in) { cudaFreeHost(h->h_obs_in); h->h_obs_in = nullptr; }
+    if (!h->obs_ev) CU(cudaEventCreateWithFlags(&h->obs_ev, cudaEventDisableTiming));
+    h->obs_ev_pending = false;
+    const size_t B = (size_t)h->series_batch, R = (size_t)h->n_scen * h->n_rows, nl = (size_t)g.n_line;
+    auto dup = [&](const void *src, size_t bytes, void **dst) -> int {
+        *dst = nullptr;
+        if (!src) return 0;
+        CU(cudaMalloc(dst, bytes ? bytes : 1));
+        h->obs_allocs.push_back(*dst);
+        if (bytes) H2D(*dst, src, bytes);
+        return 0;
+    };
+    auto zeros = [&](size_t bytes, int byte, void **dst) -> int {
+        CU(cudaMalloc(dst, bytes ? bytes : 1));
+        h->obs_allocs.push_back(*dst);
+        CU(cudaMemsetAsync(*dst, byte, bytes ? bytes : 1, h->stream));
+        return 0;
+    };
+    ObsArgs a{};
+    void *p[17] = {};
+    int rc;
+    if ((rc = dup(d->seg, (size_t)d->n_seg * 12, &p[0])) || (rc = dup(d->calendar, R * 24, &p[1])) || (rc = dup(d->max_step, (size_t)h->n_scen * 4, &p[2])) ||
+        (rc = dup(d->maint_time, R * nl * 4, &p[3])) || (rc = dup(d->maint_dur, R * nl * 4, &p[4])) ||
+        (rc = dup(d->gen_pmin, (size_t)g.n_gen * 4, &p[5])) || (rc = dup(d->gen_pmax, (size_t)g.n_gen * 4, &p[6])) ||
+        (rc = dup(d->gen_ramp_up, (size_t)g.n_gen * 4, &p[7])) || (rc = dup(d->gen_ramp_down, (size_t)g.n_gen * 4, &p[8])) ||
+        (rc = dup(d->gen_cost, (size_t)g.n_gen * 4, &p[9])) || (rc = dup(d->gen_renewable, (size_t)g.n_gen, &p[10])) ||
+        (rc = dup(d->sto_charge0, (size_t)g.n_sto * 4, &p[11])) || (rc = dup(d->sto_loss_step, (size_t)g.n_sto * 4, &p[12])) ||
+        (rc = zeros(B * nl * 4, 0, &p[13])) || (rc = zeros(B * nl * 4, 0, &p[14])) || (rc = zeros(B * 4, 0xff, &p[15])) || (rc = zeros(B * 4, 0xff, &p[16])))
+        return rc;
+    a.seg = (const int32_t *)p[0]; a.calendar = (const int32_t *)p[1]; a.max_step = (const int32_t *)p[2];
+    a.maint_time = (const int32_t *)p[3]; a.maint_dur = (const int32_t *)p[4];
+    a.gen_pmin = (const float *)p[5]; a.gen_pmax = (const float *)p[6]; a.gen_ramp_up = (const float *)p[7]; a.gen_ramp_down = (const float *)p[8];
+    a.gen_cost = (const float *)p[9]; a.gen_renewable = (const int8_t *)p[10];
+    a.sto_charge0 = (const float *)p[11]; a.sto_loss_step = (const float *)p[12];
+    a.ts_over = (int32_t *)p[13]; a.ts_prot = (int32_t *)p[14]; a.stamp = (int32_t *)p[15]; a.go_row = (int32_t *)p[16];
+    a.n_seg = d->n_seg; a.n_obs = d->n_obs; a.delta_time = d->delta_time; a.redisp_available = d->redisp_available;
+    a.reward_kind = d->reward_kind; a.max_regret = d->max_regret; a.reward_min = d->reward_min; a.reward_illegal = d->reward_illegal;
+    a.dts_hours = d->dts_hours; a.soft_thr = d->soft_thr;
+    a.host_stride = g.n_line + g.n_sub + 3;
+    if (cudaMallocHost(&h->h_obs_in, B * a.host_stride * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
+    void *din = nullptr;
+    if ((rc = zeros(B * a.host_stride * 4, 0, &din))) return rc;
+    h->d_obs_in = (int32_t *)din;
+    CU(cudaStreamSynchronize(h->stream));
+    h->obs = a; h->obs_batch = h->series_batch; h->obs_rows = h->n_rows;
+    return 0;
+}
+
+extern "C" int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float *d_reward) {
+    if (!h || !host_in || !d_obs) return fail(B200PF_E_ARG, "null pointer");
+    if (!h->obs_batch || h->obs_batch != h->series_batch || h->obs_rows != h->n_rows)
+        return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
+    CU(cudaSetDevice(h->device));
+    const DevGrid &g = h->g;
+    ObsArgs a = h->obs;
+    const size_t in_bytes = (size_t)h->obs_batch * a.host_stride * 4;
+    if (h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));        // the previous copy out of the pinned record has left
+    memcpy(h->h_obs_in, host_in, in_bytes);
+    CU(cudaMemcpyAsync(h->d_obs_in, h->h_obs_in, in_bytes, cudaMemcpyHostToDevice, h->stream));
+    CU(cudaEventRecord(h->obs_ev, h->stream));
+    h->obs_ev_pending = true;
+    a.batch = h->obs_batch;
+    a.n_line = g.n_line; a.n_sub = g.n_sub; a.n_gen = g.n_gen; a.n_hidden = g.n_hidden; a.n_load = g.n_load; a.n_sto = g.n_sto;
+    a.n_shunt = g.n_shunt; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_out = g.n_out;
+    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
+    a.out = h->x_out ? h->x_out : h->d_out; a.rho = h->x_rho ? h->x_rho : h->d_rho; a.topo = h->d_series_topo;
+    a.t = h->d_t; a.scen = h->d_scen; a.chron = h->d_chron; a.n_rows = h->n_rows; a.th_lim = h->d_thlim;
+    a.host = h->d_obs_in; a.obs = d_obs; a.reward = d_reward;
+    pf_kernel_observe<<<(a.batch + 3) / 4, 128, 0, h->stream>>>(a);
+    CU(cudaGetLastError());
+    h->obs_launches++; h->obs_h2d_bytes += (int64_t)in_bytes;
+    return 0;
+}
+
+extern "C" int b200pf_obs_stats(const b200pf_handle *h, int64_t *out4) {
+    if (!h || !out4) return fail(B200PF_E_ARG, "null pointer");
+    out4[0] = h->obs_launches; out4[1] = h->obs_h2d_bytes; out4[2] = h->d2h_bytes;
+    out4[3] = (int64_t)h->obs_batch * ((int64_t)h->obs.n_obs * 4 + (h->obs.reward_kind ? 4 : 0));
     return 0;
 }
 

@@ -36,7 +36,7 @@ ABI_SYMBOLS = (
     "b200pf_rows_group_config", "b200pf_set_kernel_policy", "b200pf_plan_stats", "b200pf_run_device_topo",
     "b200pf_set_debug", "b200pf_redo_launch_count",
     "b200pf_device_alloc", "b200pf_device_free", "b200pf_ipc_export", "b200pf_ipc_open", "b200pf_ipc_close", "b200pf_device_read", "b200pf_plan_counters", "b200pf_series_bind_flag",
-    "b200pf_series_reset_instances", "b200pf_grid_max_active_buses",
+    "b200pf_series_reset_instances", "b200pf_grid_max_active_buses", "b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats",
 )
 
 
@@ -60,6 +60,51 @@ class _GridDesc(C.Structure):
         ("shunt_sub", C.c_void_p), ("shunt_vn", C.c_void_p), ("shunt_vratio", C.c_void_p),
         ("sub_rank", C.c_void_p),
     ]
+
+
+class ObsDesc(C.Structure):
+    """``b200pf_obs_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("n_seg", C.c_int32), ("n_obs", C.c_int32), ("seg", C.c_void_p), ("calendar", C.c_void_p), ("max_step", C.c_void_p),
+        ("delta_time", C.c_float), ("maint_time", C.c_void_p), ("maint_dur", C.c_void_p),
+        ("gen_pmin", C.c_void_p), ("gen_pmax", C.c_void_p), ("gen_ramp_up", C.c_void_p), ("gen_ramp_down", C.c_void_p),
+        ("gen_cost", C.c_void_p), ("gen_renewable", C.c_void_p), ("redisp_available", C.c_int32),
+        ("sto_charge0", C.c_void_p), ("sto_loss_step", C.c_void_p), ("reward_kind", C.c_int32),
+        ("max_regret", C.c_double), ("reward_min", C.c_double), ("reward_illegal", C.c_double), ("dts_hours", C.c_double),
+        ("soft_thr", C.c_float),
+    ]
+
+
+def make_obs_desc(t: dict):
+    """-> (``b200pf_obs_desc`` for the tables ``t`` built by ``BatchedEnv.enable_observation``, the arrays it points to)"""
+    keep = []
+    d = ObsDesc()
+
+    def put(name, arr, dtype):
+        if arr is None:
+            setattr(d, name, None)
+            return
+        a = np.ascontiguousarray(arr, dtype=dtype)
+        if a.size == 0:
+            a = np.zeros(1, dtype=dtype)
+        keep.append(a)
+        setattr(d, name, a.ctypes.data)
+
+    d.n_seg, d.n_obs = len(t["seg"]), int(t["n_obs"])
+    put("seg", t["seg"], np.int32); put("calendar", t["calendar"], np.int32); put("max_step", t["max_step"], np.int32)
+    d.delta_time = float(t["delta_time"])
+    put("maint_time", t.get("maint_time"), np.int32); put("maint_dur", t.get("maint_dur"), np.int32)
+    g = t["gen"]
+    put("gen_pmin", g["gen_pmin"], np.float32); put("gen_pmax", g["gen_pmax"], np.float32)
+    put("gen_ramp_up", g["gen_max_ramp_up"], np.float32); put("gen_ramp_down", g["gen_max_ramp_down"], np.float32)
+    put("gen_cost", g["gen_cost_per_MW"], np.float32); put("gen_renewable", g["gen_renewable"], np.int8)
+    d.redisp_available = int(bool(g["available"]))
+    put("sto_charge0", t["storage"]["charge0"], np.float32); put("sto_loss_step", t["storage"]["loss_step"], np.float32)
+    d.reward_kind = int(t["reward_kind"])
+    r = t["reward"]
+    d.max_regret, d.reward_min, d.reward_illegal, d.dts_hours = r["max_regret"], r["reward_min"], r["reward_illegal"], r["dts_hours"]
+    d.soft_thr = float(t["soft_thr"])
+    return d, keep
 
 
 def lib_path() -> str:
@@ -138,6 +183,11 @@ def load_library():
     lib.b200pf_device_read.argtypes = [vp, vp, C.c_size_t]
     lib.b200pf_device_read.restype = i32
     for nm in ("b200pf_set_debug", "b200pf_device_alloc", "b200pf_device_free", "b200pf_ipc_export", "b200pf_ipc_open", "b200pf_ipc_close"):
+        getattr(lib, nm).restype = i32
+    lib.b200pf_obs_bind.argtypes = [vp, C.POINTER(ObsDesc)]
+    lib.b200pf_observe.argtypes = [vp, vp, vp, vp]
+    lib.b200pf_obs_stats.argtypes = [vp, C.POINTER(C.c_int64)]
+    for nm in ("b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -277,6 +327,7 @@ class PowerFlowEngine:
 
     def __init__(self, gm: GridModel, max_batch: int = 1, device: int = 0):
         self.gm = gm
+        self.device = int(device)
         self.lib = load_library()
         if self.lib.b200pf_abi_version() != 2:
             raise EngineUnavailable("libb200pf ABI version mismatch")
@@ -535,6 +586,24 @@ class PowerFlowEngine:
         p = [C.c_void_p() for _ in range(5)]
         self._check(self.lib.b200pf_series_results(self.h, *[C.byref(v) for v in p]), "b200pf_series_results")
         return dict(out=p[0].value, status=p[1].value, iters=p[2].value, rho=p[3].value, t=p[4].value)
+
+    # ---- observation layer -------------------------------------------------------------------
+    def obs_bind(self, tables: dict):
+        """Static tables of the observation layer for the bound series (``b200pf_obs_bind``; built by BatchedEnv.enable_observation)."""
+        d, keep = make_obs_desc(tables)
+        self._check(self.lib.b200pf_obs_bind(self.h, C.byref(d)), "b200pf_obs_bind")
+        del keep
+
+    def observe(self, host_in: np.ndarray, d_obs: int, d_reward: int = 0):
+        """Asynchronous on the handle's stream: H2D of the per-instance host inputs (int32 [batch, n_line + n_sub + 3]), one launch
+        writing obs f32 [batch, n_obs] / reward f32 [batch] to the DEVICE pointers ``d_obs`` / ``d_reward``."""
+        h = np.ascontiguousarray(host_in, dtype=np.int32)
+        self._check(self.lib.b200pf_observe(self.h, _ptr(h), C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe")
+
+    def obs_stats(self):
+        v = (C.c_int64 * 4)()
+        self._check(self.lib.b200pf_obs_stats(self.h, v), "b200pf_obs_stats")
+        return dict(launches=int(v[0]), h2d_bytes=int(v[1]), d2h_bytes=int(v[2]), bytes_written_per_launch=int(v[3]))
 
     def sync(self):
         self._check(self.lib.b200pf_sync(self.h), "b200pf_sync")

@@ -291,6 +291,44 @@ int b200pf_ipc_close(void *d_ptr);
 int b200pf_set_debug(b200pf_handle *h, int planned_div_mod, int redo_enabled);
 int64_t b200pf_redo_launch_count(const b200pf_handle *h);
 
+/* Observation layer: grid2op observation vectors (obs.to_vect(), every attribute as float32) and rewards for the whole bound
+ * series, assembled on the device from what a series step leaves there (result records, rho, device topology, chronics row
+ * index) — no device-to-host copy of the result records.  b200pf_obs_bind copies the static tables below (host pointers) and
+ * clears the overflow counters the layer keeps (timestep_overflow / timestep_protection_engaged, reference
+ * grid2op/Environment/baseEnv.py:3361-3370, counted whether the protections are on or not); a re-bound series needs a new
+ * b200pf_obs_bind.  The attribute sources of `seg` are enum ObsSrc of csrc/b200pf_obs.cuh (grid2op_b200/observation.py builds them
+ * from attribute names).
+ * b200pf_observe enqueues, on the handle's stream and behind the last series step, one H2D copy of the per-instance host inputs
+ * (from a pinned buffer of the handle) and one launch (a warp per instance) writing obs f32 [batch][n_obs] and reward f32 [batch]
+ * into caller-owned DEVICE buffers (torch tensors, like b200pf_series_bind_outputs; reward may be NULL).  host_in: int32
+ * [batch][n_line + n_sub + 3] = time_before_cooldown_line | time_before_cooldown_sub | current_step | stamp | flags — 4 (n_line +
+ * n_sub + 3) bytes per instance.  The counters advance once per distinct stamp (the caller's step number): observe after every
+ * step.  flags: B200PF_OBS_ILLEGAL (the step's action was replaced by "do nothing"), B200PF_OBS_DONE (the instance is game over:
+ * the game-over observation of BaseObservation.set_game_over, baseObservation.py:1551, and reward_min), B200PF_OBS_RESET (the
+ * instance was reset: its counters restart from 0). */
+enum { B200PF_REWARD_NONE = 0, B200PF_REWARD_REDISP = 1, B200PF_REWARD_L2RPN = 2 };
+enum { B200PF_OBS_ILLEGAL = 1, B200PF_OBS_DONE = 2, B200PF_OBS_RESET = 4 };
+typedef struct b200pf_obs_desc {
+    int32_t n_seg, n_obs;
+    const int32_t *seg;                 /* [n_seg][3]: attribute source, offset in the vector, length */
+    const int32_t *calendar;            /* [n_scen][n_rows][6] year month day hour minute weekday(Monday = 0) of every row */
+    const int32_t *max_step;            /* [n_scen] */
+    float delta_time;                   /* minutes */
+    const int32_t *maint_time, *maint_dur; /* [n_scen][n_rows][n_line] or NULL: time_next_maintenance / duration_next_maintenance */
+    const float *gen_pmin, *gen_pmax, *gen_ramp_up, *gen_ramp_down, *gen_cost;  /* [n_gen] (prods_charac.csv) */
+    const int8_t *gen_renewable;        /* [n_gen] */
+    int32_t redisp_available;
+    const float *sto_charge0, *sto_loss_step;  /* [n_storage] MWh: charge after the reset step, loss withdrawn per step */
+    int32_t reward_kind;                /* B200PF_REWARD_* */
+    double max_regret, reward_min, reward_illegal, dts_hours;   /* RedispReward constants; step length in hours */
+    float soft_thr;                     /* SOFT_OVERFLOW_THRESHOLD (timestep_protection_engaged) */
+} b200pf_obs_desc;
+int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *desc);
+int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float *d_reward);
+/* out4 = { observe launches, bytes of their host inputs copied H2D, bytes this handle copied device-to-host since create (series
+ * fetch / fetch_state), bytes one observe launch writes } */
+int b200pf_obs_stats(const b200pf_handle *h, int64_t *out4);
+
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */
 uint64_t b200pf_stream(b200pf_handle *h);
