@@ -145,6 +145,19 @@ extern "C" int b200pf_device_count(void) {
     return n;
 }
 
+#if PB_CLOCK_ON
+// Measurement build only (-DB200PF_PHASE_CLOCK): copies the block kernel's phase clock (b200pf_block.cuh, PC_SLOTS counters
+// of the current device) to dst after a device synchronise, then clears it.  Not part of the ABI of include/b200pf.h.
+extern "C" int b200pf_phase_clock_read(unsigned long long *dst, int n) {
+    if (!dst || n < PC_SLOTS) return fail(B200PF_E_ARG, "phase clock: destination too small");
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpyFromSymbol(dst, pb_phase_clk, sizeof(unsigned long long) * PC_SLOTS));
+    static const unsigned long long zeros[PC_SLOTS] = {};
+    CU(cudaMemcpyToSymbol(pb_phase_clk, zeros, sizeof(zeros)));
+    return PC_SLOTS;
+}
+#endif
+
 extern "C" int b200pf_create(const b200pf_grid_desc *gd, int max_batch, int device, b200pf_handle **out) {
     if (!gd || !out || max_batch <= 0) return fail(B200PF_E_ARG, "null argument or max_batch <= 0");
     if (gd->abi_version != B200PF_ABI_VERSION) return fail(B200PF_E_ARG, "ABI version mismatch");
@@ -859,8 +872,15 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     constexpr int BLOCK = (T < 32 ? 32 : T) * WPC;
     auto kern = pf_kernel_block<T, U, MINB, PROT, WPC, STAGE, UNI, MODE>;
     const int ws = sel.smem * G;                         // workspace of one warp / CTA
-    int plan_bytes = 0;
-    if (STAGE) plan_bytes = reinterpret_cast<const PlanHeader *>(h->plan_blobs.data() + h->plan_off[sel.single])->total_bytes;
+    int plan_bytes = 0, row_ahead = 0;
+    const unsigned char *plan_src = nullptr;
+    if (STAGE) {
+        // (the kernel starts the plan's bulk copy from its address and, for a solvable plan, loads the chronics rows meanwhile)
+        const PlanHeader *H = reinterpret_cast<const PlanHeader *>(h->plan_blobs.data() + h->plan_off[sel.single]);
+        plan_bytes = H->total_bytes;
+        plan_src = h->d_plan_blobs + h->plan_off[sel.single];
+        row_ahead = H->status == PLAN_ST_OK;        // (one plan: sel.lay_nb / lay_nblkA are its sizes, sel_layout)
+    }
     if (STAGE) { int rc = stat_sync(h); if (rc) return rc; }
     const int smem = ws * WPC + plan_bytes + (STAGE ? h->stat_off.total : 0);
     const int variant = 1000 + MINB * 4096 + T * 64 + U * 8 + (PROT ? 1 : 0) + (STAGE ? 2 : 0) + (WPC > 1 ? 4 : 0) + (UNI ? 100000 : 0) + MODE * 200000;
@@ -891,7 +911,7 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     const int rounds = (n_cta_work + resident - 1) / resident;
     int grid = (n_cta_work + rounds - 1) / rounds;
     if (grid < 1) grid = 1;
-    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(g, a, pa, ws, plan_bytes);
+    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(g, a, pa, ws, plan_bytes, plan_src, row_ahead);
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 4;

@@ -32,6 +32,8 @@ namespace b200pf {
 #else
 #define PB_UNROLL _Pragma("unroll")
 #define PB_LOOP _Pragma("unroll 1")      // the lane loops run 1-3 times: unrolled copies only cost instruction-cache misses (ncu: no_inst 15 %)
+// (also the per-bus element lists of the code that runs once per solve: 0-3 entries, and that code is fetched cold after an
+// L2 flush; with the staged arrays known to be shared memory the compiler unrolls each of them 4x)
 // UNI ("lockstep"): all instances of the warp share one plan and run the same control flow, so the whole warp
 // synchronises with the plain full-mask primitives.  A per-lane mask (instances free to diverge) makes every barrier / vote a
 // MATCH-based collective.
@@ -44,6 +46,26 @@ template <int T, int G, bool UNI> __device__ __forceinline__ int pb_any(unsigned
 }
 #define PB_SYNC() pb_sync<T, G, UNI>(imask)
 #define PB_ANY(x) pb_any<T, G, UNI>(imask, (x))
+#endif
+
+#if defined(B200PF_PHASE_CLOCK) && !defined(B200PF_EMULATE)
+// Measurement build only (-DB200PF_PHASE_CLOCK, scripts/phase_clock.py); the production build compiles none of this.
+// Lane 0 of every warp adds the SM cycles (clock64) spent between consecutive phase boundaries of solve_block to
+// pb_phase_clk[phase] (summed over the Newton iterations, the warps and the launches until the host reads and clears it);
+// pf_kernel_block adds every warp's cycle and globaltimer spans, from which the host converts cycles to time.
+enum { PC_STAGE, PC_ROW, PC_SUMS, PC_DCINV, PC_DCANG, PC_LINES, PC_BUSES, PC_STREAM, PC_UPDATE, PC_OUT, PC_N_PHASE,
+       PC_SOLVES = PC_N_PHASE, PC_WARPS, PC_CYCLES, PC_NS, PC_SLOTS };
+__device__ unsigned long long pb_phase_clk[PC_SLOTS];
+#define PB_CLOCK_ON 1
+#define PB_CLOCK(k)                                                                                                   \
+    {                                                                                                                 \
+        const long long t_ = clock64();                                                                               \
+        if (clk_lane0) atomicAdd(&pb_phase_clk[k], (unsigned long long)(t_ - clk_last));                             \
+        clk_last = t_;                                                                                                \
+    }
+#else
+#define PB_CLOCK_ON 0
+#define PB_CLOCK(k)
 #endif
 
 template <int T, int G, bool UNI = false>
@@ -63,17 +85,15 @@ PF_DEV void block_fail(const DevGrid &g, const RunArgs &a, int inst, int status,
     (void)tid0; (void)imask;
 }
 
-// sm: workspace of the WARP (G instances, interleaved); gi: instance slot of this lane in the warp; tid0: lane of the instance
-// MODE 1: AC solve fed by chronics rows (series / rows entry points) known at compile time — the DC branches and the fp64-record
-// input paths drop out of the kernel (ncu: 13 % of the stall samples at batch 4096 were instruction-fetch stalls); 0: generic
-template <int T, int U, int G, bool PROT, bool UNI = false, int MODE = 0>
-PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int gi, int tid0, unsigned imask) {
+// The chronics row an instance solves, from the kernel arguments alone (no plan needed): series entry point -> row a.t[src]
+// of scenario a.scen[src], and a.t[inst] advances for the next step; rows entry point -> row src of a.rows.  nullptr: the
+// instance reads an fp64 injection record instead (MODE 0 without a series).
+template <int T, int G, bool PROT, bool UNI, int MODE>
+PF_DEV const float *block_row(const DevGrid &g, const RunArgs &a, int inst, int tid0, unsigned imask) {
 #ifndef B200PF_EMULATE
     const int tid = tid0;
 #endif
     const int src = a.n1_lines > 0 ? inst / a.n1_lines : inst;          // record the inputs come from
-    const unsigned char *blob = pa.blobs + pa.plan_off[pa.inst_plan ? pa.inst_plan[inst] : 0];
-    const PlanHeader &H = *reinterpret_cast<const PlanHeader *>(blob);
     int trow = 0, sc = 0;
     if (a.series && !a.rows) {
         sc = a.scen[src]; trow = a.t[src];
@@ -81,6 +101,49 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         if (PROT && a.casc > 0) trow = trow == 0 ? a.n_rows - 1 : trow - 1;       // later cascade rounds re-solve the SAME row
         PF_PHASE { if (tid == 0 && a.n1_lines <= 0 && !(PROT && a.casc > 0)) a.t[inst] = (trow + 1 >= a.n_rows) ? 0 : trow + 1; }
     }
+    (void)tid0; (void)imask;
+    if (!(MODE == 1 || a.series != 0)) return nullptr;
+    const size_t n_row = (size_t)(2 * g.n_load + 2 * g.n_gen);
+    return a.rows ? a.rows + (size_t)src * n_row : a.chron + ((size_t)sc * a.n_rows + trow) * n_row;
+}
+
+// the row into the instance's interleaved copy srow of the warp's workspace
+template <int T, int G, bool UNI>
+PF_DEV void block_row_copy(const float *grow, int n, float *srow, int gi, int tid0, unsigned imask) {
+#ifndef B200PF_EMULATE
+    const int tid = tid0;
+#endif
+    PF_PHASE { for (int k = tid; k < n; k += T) srow[k * G + gi] = grow[k]; }
+    PB_SYNC();
+    (void)tid0; (void)imask;
+}
+
+// Byte offset of srow in a warp's workspace (the layout solve_block builds from the strides Lnb / LnblkA): value blocks, six
+// bus arrays, the shunt pair, V, the branch currents, then the row.
+template <int G>
+PF_DEV size_t block_srow_off(int Lnb, int LnblkA, int nsh, int nl) {
+    const size_t Lb = (size_t)Lnb * G, LA = (size_t)(LnblkA + 1) * G;
+    return LA * 16 + (6 * Lb + 2 * (size_t)nsh * G) * 8 + (Lb + 2 * (size_t)nl * G) * 16;
+}
+
+// sm: workspace of the WARP (G instances, interleaved); gi: instance slot of this lane in the warp; tid0: lane of the instance
+// MODE 1: AC solve fed by chronics rows (series / rows entry points) known at compile time — the DC branches and the fp64-record
+// input paths drop out of the kernel (ncu: 13 % of the stall samples at batch 4096 were instruction-fetch stalls); 0: generic
+// STAGE: the plan (and pa.stat) are the launch's copies in shared memory, and the kernel has already run block_row /
+// block_row_copy for this instance (for its first instance group while the plan's bulk copy was in flight).
+template <int T, int U, int G, bool PROT, bool UNI = false, int MODE = 0, bool STAGE = false>
+PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int gi, int tid0, unsigned imask) {
+#ifndef B200PF_EMULATE
+    const int tid = tid0;
+#endif
+#if PB_CLOCK_ON
+    const bool clk_lane0 = tid0 == 0 && gi == 0;
+    long long clk_last = clock64();
+#endif
+    const int src = a.n1_lines > 0 ? inst / a.n1_lines : inst;          // record the inputs come from
+    const unsigned char *blob = pa.blobs + pa.plan_off[pa.inst_plan ? pa.inst_plan[inst] : 0];
+    const PlanHeader &H = *reinterpret_cast<const PlanHeader *>(blob);
+    const float *grow = STAGE ? nullptr : block_row<T, G, PROT, UNI, MODE>(g, a, inst, tid0, imask);
     // fstat >= 0: the instance has failed with this status.  Free-running instances (UNI = false) leave at once; in lockstep
     // the lanes keep executing with the warp (their state is garbage from then on) and store the failure record at the end.
     int fstat = -1, fiters = 0;
@@ -95,12 +158,12 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
 #define U16(off) reinterpret_cast<const uint16_t *>(blob + H.off)
 #define F64(off) reinterpret_cast<const double *>(blob + H.off)
 #define IX(i) ((i) * G + gi)
-#define PB_STAT(name, type) const type *name##_ = pa.stat ? reinterpret_cast<const type *>(pa.stat + pa.so.name) : g.name;
+#define PB_STAT(name, type) const type *name##_ = STAGE ? reinterpret_cast<const type *>(pa.stat + pa.so.name) : g.name;
     PB_STAT(line_y, double) PB_STAT(line_bdc, double) PB_STAT(line_pshift, double) PB_STAT(line_or_vn, float) PB_STAT(line_ex_vn, float)
     PB_STAT(unit_is_ref, int) PB_STAT(unit_qmin, double) PB_STAT(unit_qmax, double) PB_STAT(unit_vn, float) PB_STAT(load_vn, float)
     PB_STAT(sto_vn, float) PB_STAT(sto_q, double) PB_STAT(sh_vn, float) PB_STAT(sh_vratio, double)
 #undef PB_STAT
-    const float *th_lim_ = pa.stat ? reinterpret_cast<const float *>(pa.stat + pa.so.th_lim) : a.th_lim;
+    const float *th_lim_ = STAGE ? reinterpret_cast<const float *>(pa.stat + pa.so.th_lim) : a.th_lim;
     const double *line_y = line_y_;
     const uint16_t *p_colth = U16(o_colth), *p_colv = U16(o_colv), *p_dcidx = U16(o_dcidx);
     const uint16_t *p_brf = U16(o_brf), *p_brt = U16(o_brt);
@@ -117,13 +180,11 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
     // ---- injections of this instance ----------------------------------------------------------------------
     const bool has_row = MODE == 1 ? true : (a.series != 0);
     const bool is_dc = MODE == 1 ? false : (a.is_dc != 0);
-    const double *rec = nullptr, *si = pa.stat ? reinterpret_cast<const double *>(pa.stat + pa.so.static_inj) : a.static_inj;
+    const double *rec = nullptr, *si = STAGE ? reinterpret_cast<const double *>(pa.stat + pa.so.static_inj) : a.static_inj;
     if (has_row) {
-        const float *grow = a.rows ? a.rows + (size_t)src * (size_t)(2 * nld + 2 * ng)
-                                   : a.chron + ((size_t)sc * a.n_rows + trow) * (size_t)(2 * nld + 2 * ng);
-        PF_PHASE { for (int k = tid; k < 2 * nld + 2 * ng; k += T) srow[IX(k)] = grow[k]; }
-        PB_SYNC();
+        if (!STAGE) block_row_copy<T, G, UNI>(grow, 2 * nld + 2 * ng, srow, gi, tid0, imask);
     } else rec = a.inj + (size_t)src * g.n_inj;
+    PB_CLOCK(PC_ROW)
 #define ROW(k) srow[IX(k)]
 #define GEN_P(u) ((u) < nh ? 0.0 : (has_row ? (double)ROW(2 * nld + (u) - nh) : rec[(u) - nh]))
 #define UNIT_VM(u) (has_row ? ((u) >= nh ? (double)PF_FDIV(ROW(2 * nld + ng + (u) - nh), unit_vn_[u]) : si[ng + (u)]) : rec[ng + (u)])
@@ -142,10 +203,10 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         PF_PHASE {
             PB_LOOP for (int i = tid; i < nb; i += T) {
                 double pg = 0.0, pd = 0.0, qd = 0.0, gs = 0.0, bsu = 0.0;
-                for (int e = bu_ptr[i]; e < bu_ptr[i + 1]; ++e) { const int u = bu[e]; pg += GEN_P(u); }
-                for (int e = bl_ptr[i]; e < bl_ptr[i + 1]; ++e) { const int k = bl[e]; pd += LOAD_P(k); qd += LOAD_Q(k); }
-                for (int e = bs_ptr[i]; e < bs_ptr[i + 1]; ++e) { const int k = bs[e]; pd += STO_P(k); qd += sto_q_[k]; }
-                for (int e = bh_ptr[i]; e < bh_ptr[i + 1]; ++e) { const int k = bh[e]; gs += SH_P(k) * sh_vratio_[k]; bsu -= SH_Q(k) * sh_vratio_[k]; }
+                PB_LOOP for (int e = bu_ptr[i]; e < bu_ptr[i + 1]; ++e) { const int u = bu[e]; pg += GEN_P(u); }
+                PB_LOOP for (int e = bl_ptr[i]; e < bl_ptr[i + 1]; ++e) { const int k = bl[e]; pd += LOAD_P(k); qd += LOAD_Q(k); }
+                PB_LOOP for (int e = bs_ptr[i]; e < bs_ptr[i + 1]; ++e) { const int k = bs[e]; pd += STO_P(k); qd += sto_q_[k]; }
+                PB_LOOP for (int e = bh_ptr[i]; e < bh_ptr[i + 1]; ++e) { const int k = bh[e]; gs += SH_P(k) * sh_vratio_[k]; bsu -= SH_Q(k) * sh_vratio_[k]; }
                 const int vu = vmunit[i];
                 vm[IX(i)] = vu != 0xFFFF ? UNIT_VM(vu) : 1.0;
                 const double ps = (pg - pd) * inv_base, gpu = gs * inv_base;      // (one division per lane instead of four per bus)
@@ -158,10 +219,13 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         }
         PB_SYNC();
     }
+    PB_CLOCK(PC_SUMS)
     // ---- 2. DC angles: theta = Bdc^-1 b with the plan's fp64 inverse (lane = row; Pc = right-hand side, Qc = result) ------
     {
-        // (the inverse is streamed from global memory with evict-first loads even when the plan itself is staged in shared memory)
-        const double *inv = reinterpret_cast<const double *>((pa.stage_src ? pa.stage_src : blob) + H.o_dcinv);
+        // staged: the plan's copy in shared memory (the 8 lanes of an instance read 8 consecutive doubles, the instances of a
+        // warp the same ones: conflict free); otherwise streamed from global memory with evict-first loads
+#define PB_INV(p) (STAGE ? *(p) : PF_LDCS(p))
+        const double *inv = F64(o_dcinv);
         const int n1 = H.n1;
         PF_PHASE {
             PB_LOOP for (int i = tid; i < n1; i += T) {
@@ -169,16 +233,18 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 const double *col = inv + i;
                 int j = 0;
                 for (; j + 3 < n1; j += 4) {
-                    const double a0 = PF_LDCS(col + (size_t)j * n1), a1 = PF_LDCS(col + (size_t)(j + 1) * n1), a2 = PF_LDCS(col + (size_t)(j + 2) * n1),
-                                 a3 = PF_LDCS(col + (size_t)(j + 3) * n1);
+                    const double a0 = PB_INV(col + (size_t)j * n1), a1 = PB_INV(col + (size_t)(j + 1) * n1), a2 = PB_INV(col + (size_t)(j + 2) * n1),
+                                 a3 = PB_INV(col + (size_t)(j + 3) * n1);
                     s0 += a0 * Pc[IX(j)]; s1 += a1 * Pc[IX(j + 1)]; s2 += a2 * Pc[IX(j + 2)]; s3 += a3 * Pc[IX(j + 3)];
                 }
-                for (; j < n1; ++j) s0 += PF_LDCS(col + (size_t)j * n1) * Pc[IX(j)];
+                for (; j < n1; ++j) s0 += PB_INV(col + (size_t)j * n1) * Pc[IX(j)];
+#undef PB_INV
                 Qc[IX(i)] = (s0 + s1) + (s2 + s3);
             }
         }
         PB_SYNC();
     }
+    PB_CLOCK(PC_DCINV)
     {
         int bad = 0;
         PF_PHASE {
@@ -207,6 +273,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         bool conv = false, running = fstat < 0;
         PF_PHASE { for (int k = tid; k < n_bzero; k += T) A4[IX(bzero[k])] = make_float4(0.f, 0.f, 0.f, 0.f); }
         PB_SYNC();
+        PB_CLOCK(PC_DCANG)
         // off-diagonal blocks of line l: block (f, t) += [ti tr; -tr ti] with T = Vf conj(yft Vt), rows of a PV bus f keep only
         // the P row, columns of a PV bus t only the theta column; same for (t, f).  Two separate read-modify-writes (a line
         // with both ends on one bus hits the same block twice).
@@ -248,6 +315,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 }
             }
             PB_SYNC();
+            PB_CLOCK(PC_LINES)
             int viol = 0, wild = 0;
             PF_PHASE {                                         // lane = bus: S = V conj(I), mismatch, diagonal block, right-hand side
                 PB_LOOP for (int i = tid; i < nb; i += T) {
@@ -277,6 +345,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 }
             }
             viol = PB_ANY(viol);
+            PB_CLOCK(PC_BUSES)
 #ifndef B200PF_EMULATE
             if (UNI) {
                 // lockstep: an instance that is through (converged / given up) keeps running with the warp until all are; its
@@ -372,6 +441,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
 #endif
 #undef PB_AT
             }
+            PB_CLOCK(PC_STREAM)
             PF_PHASE {                                         // lane = bus: state update from the solved right-hand-side blocks
                 PB_LOOP for (int i = tid; i < ((!UNI || running) ? nb : 0); i += T) {
                     const int c = p_dcidx[i];
@@ -405,6 +475,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 PB_LOOP for (int k = tid; k < n_bzero; k += T) A4[IX(bzero[k])] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
             PB_SYNC();
+            PB_CLOCK(PC_UPDATE)
         }
 #undef PB_OFFDIAG
         if (!conv) PB_FAIL(ST_DIV, iters)
@@ -481,9 +552,9 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                     const int i = unit_bus[u];
                     if (i != 0xFFFF) {
                         double pd = 0.0, qd = 0.0, pnonref = 0.0;
-                        for (int e = bl_ptr[i]; e < bl_ptr[i + 1]; ++e) { const int k = bl[e]; pd += LOAD_P(k); qd += LOAD_Q(k); }
-                        for (int e = bs_ptr[i]; e < bs_ptr[i + 1]; ++e) { const int k = bs[e]; pd += STO_P(k); qd += sto_q_[k]; }
-                        for (int e = bu_ptr[i]; e < bu_ptr[i + 1]; ++e) { const int u2 = bu[e]; if (!unit_is_ref_[u2]) pnonref += GEN_P(u2); }
+                        PB_LOOP for (int e = bl_ptr[i]; e < bl_ptr[i + 1]; ++e) { const int k = bl[e]; pd += LOAD_P(k); qd += LOAD_Q(k); }
+                        PB_LOOP for (int e = bs_ptr[i]; e < bs_ptr[i + 1]; ++e) { const int k = bs[e]; pd += STO_P(k); qd += sto_q_[k]; }
+                        PB_LOOP for (int e = bu_ptr[i]; e < bu_ptr[i + 1]; ++e) { const int u2 = bu[e]; if (!unit_is_ref_[u2]) pnonref += GEN_P(u2); }
                         double pu = GEN_P(u);
                         if (unit_is_ref_[u]) pu = (Pc[IX(i)] * base + pd - pnonref) / (double)p_nref[i];     // slack share (pandapower pfsoln)
                         double qu = 0.0;
@@ -527,10 +598,14 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         PB_SYNC();
         if (a.busv) {
             double *bv = a.busv + (size_t)inst * 2 * g.n_slot;
-            PF_PHASE { if (!(UNI && fstat >= 0)) for (int i = tid; i < nb; i += T) { bv[p_slot[i]] = vm[IX(i)]; bv[g.n_slot + p_slot[i]] = va[IX(i)]; } }
+            PF_PHASE { if (!(UNI && fstat >= 0)) PB_LOOP for (int i = tid; i < nb; i += T) { bv[p_slot[i]] = vm[IX(i)]; bv[g.n_slot + p_slot[i]] = va[IX(i)]; } }
             PB_SYNC();
         }
     }
+    PB_CLOCK(PC_OUT)
+#if PB_CLOCK_ON
+    if (clk_lane0) atomicAdd(&pb_phase_clk[PC_SOLVES], 1ull);
+#endif
     if (PROT) {
         // Cascading-failure round: same rules and bookkeeping as the PROT block of solve_sparse (reference
         // Backend.next_grid_state, backend.py:1466-1521; counters baseEnv.py:3361-3370)
@@ -595,8 +670,9 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
 // re-reading the index arrays and the operation stream through L1 for every instance (B200PF_BLOCK_STAGE=0 selects the L1
 // path for comparison).
 __device__ __forceinline__ uint32_t pb_smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void pb_stage(unsigned char *dst, const unsigned char *src, uint32_t bytes, unsigned char *dst2, const unsigned char *src2,
-                                         uint32_t bytes2, uint64_t *mbar) {
+// starts the two copies (the CTA's first barrier included); pb_stage_wait returns once both have landed
+__device__ __forceinline__ void pb_stage_issue(unsigned char *dst, const unsigned char *src, uint32_t bytes, unsigned char *dst2,
+                                               const unsigned char *src2, uint32_t bytes2, uint64_t *mbar) {
     const uint32_t mb = pb_smem_addr(mbar);
     if (threadIdx.x == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(mb), "r"(1) : "memory");
@@ -610,6 +686,9 @@ __device__ __forceinline__ void pb_stage(unsigned char *dst, const unsigned char
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(pb_smem_addr(dst2)), "l"(src2), "r"(bytes2), "r"(mb) : "memory");
     }
+}
+__device__ __forceinline__ void pb_stage_wait(uint64_t *mbar) {
+    const uint32_t mb = pb_smem_addr(mbar);
     uint32_t ok = 0;
     while (!ok) {
         asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
@@ -619,15 +698,26 @@ __device__ __forceinline__ void pb_stage(unsigned char *dst, const unsigned char
 
 // WPC warps per CTA for T <= 32 (each warp: G = 32 / T instances interleaved), one CTA of T threads per instance beyond.
 // Persistent: warp slot w of CTA c takes the instance groups c * WPC + w, + gridDim * WPC, ...
-// ws_bytes: workspace of one warp; STAGE: the launch's single plan is copied behind the workspaces first (plan_bytes).
+// ws_bytes: workspace of one warp; STAGE: the launch's single plan (plan_bytes at plan_src in global memory) is copied behind
+// the workspaces first, and while that copy is in flight every warp loads the chronics rows of its first instance group
+// (row_ahead = 1: the plan is a solvable one, so pa_in.lay_nb / lay_nblkA give the workspace layout without its header;
+// 0: solve_block stops at the plan's status before it reads a row, only a.t advances).
 // UNI (T < 32 only): lockstep warps — requires ONE plan for the launch and batch % G == 0 (the host checks both).
 template <int T, int U, int MINB, bool PROT, int WPC = 1, bool STAGE = false, bool UNI = false, int MODE = 0>
 __global__ void __launch_bounds__((T < 32 ? 32 : T) * WPC, MINB)
-pf_kernel_block(const DevGrid g, const RunArgs a, const PlanArgs pa_in, const int ws_bytes, const int plan_bytes) {
+pf_kernel_block(const DevGrid g, const RunArgs a, const PlanArgs pa_in, const int ws_bytes, const int plan_bytes, const unsigned char *plan_src,
+                const int row_ahead) {
     extern __shared__ __align__(16) unsigned char smem[];
     // the safety-net kernel behind this launch (programmatic dependent launch) may be set up right away: it parks at its
     // griddepcontrol.wait until this grid has completed, so its launch latency is off the critical path
     asm volatile("griddepcontrol.launch_dependents;");
+#if PB_CLOCK_ON
+    const bool clk_lane0 = (threadIdx.x & 31) == 0;
+    const long long clk_entry = clock64();
+    long long clk_last = clk_entry;
+    unsigned long long gt_entry;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_entry));
+#endif
     constexpr int G = T < 32 ? 32 / T : 1;
     static_assert(WPC == 1 || T <= 32, "several instances groups per CTA only for warp-sized groups");
     const int lane = T <= 32 ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
@@ -645,27 +735,47 @@ pf_kernel_block(const DevGrid g, const RunArgs a, const PlanArgs pa_in, const in
     if (!STAGE) pa.stat = nullptr;
     __shared__ int zero_off;
     __shared__ __align__(8) uint64_t mbar;
+    unsigned char *ws = smem + (size_t)warp * ws_bytes;
+    const int n_grp = (a.batch + G - 1) / G;
+    // staged launches: the inputs of an instance group (its chronics rows; the advance of a.t) are loaded here, ahead of
+    // solve_block — for the warp's first group while the plan's bulk copy is in flight
+    auto load_rows = [&](int inst) {
+        const float *grow = block_row<T, G, PROT, UNI, MODE>(g, a, inst, j, imask);
+        if (grow && row_ahead)
+            block_row_copy<T, G, UNI>(grow, 2 * g.n_load + 2 * g.n_gen,
+                                      reinterpret_cast<float *>(ws + block_srow_off<G>(pa_in.lay_nb, pa_in.lay_nblkA, g.n_shunt, g.n_line)), gi, j, imask);
+    };
+    int w = blockIdx.x * WPC + warp;
     if (STAGE) {
         // behind the workspaces: the plan blob, then the blob of static grid arrays (pa_in.stat: its copy in global memory)
         unsigned char *dst = smem + (size_t)WPC * ws_bytes;
         unsigned char *dst2 = dst + plan_bytes;
-        pb_stage(dst, pa_in.blobs + pa_in.plan_off[0], (uint32_t)plan_bytes, dst2, pa_in.stat, (uint32_t)pa_in.so.total, &mbar);
+        if (threadIdx.x == 0) zero_off = 0;             // (published by the barrier inside pb_stage_issue)
+        pb_stage_issue(dst, plan_src, (uint32_t)plan_bytes, dst2, pa_in.stat, (uint32_t)pa_in.so.total, &mbar);
+        if (w < n_grp && w * G + gi < a.batch) load_rows((PROT && a.inst_list) ? a.inst_list[w * G + gi] : w * G + gi);
+        pb_stage_wait(&mbar);
         pa.stat = dst2;
-        if (threadIdx.x == 0) zero_off = 0;
-        __syncthreads();
-        pa.stage_src = pa_in.blobs + pa_in.plan_off[0];
         pa.blobs = dst; pa.plan_off = &zero_off; pa.inst_plan = nullptr;
     }
-    unsigned char *ws = smem + (size_t)warp * ws_bytes;
-    const int n_grp = (a.batch + G - 1) / G;
-    for (int w = blockIdx.x * WPC + warp; w < n_grp; w += gridDim.x * WPC) {
+    PB_CLOCK(PC_STAGE)
+    for (bool first = true; w < n_grp; w += gridDim.x * WPC, first = false) {
         const int k = w * G + gi;
         if (k < a.batch) {
             const int inst = (PROT && a.inst_list) ? a.inst_list[k] : k;
-            solve_block<T, U, G, PROT, UNI, MODE>(g, a, pa, inst, ws, gi, j, imask);
+            if (STAGE && !first) load_rows(inst);
+            solve_block<T, U, G, PROT, UNI, MODE, STAGE>(g, a, pa, inst, ws, gi, j, imask);
         }
         if (T <= 32) __syncwarp(); else __syncthreads();
     }
+#if PB_CLOCK_ON
+    if (clk_lane0) {
+        unsigned long long gt_end;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_end));
+        atomicAdd(&pb_phase_clk[PC_WARPS], 1ull);
+        atomicAdd(&pb_phase_clk[PC_CYCLES], (unsigned long long)(clock64() - clk_entry));
+        atomicAdd(&pb_phase_clk[PC_NS], gt_end - gt_entry);
+    }
+#endif
 }
 #endif
 

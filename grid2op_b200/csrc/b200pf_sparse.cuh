@@ -118,7 +118,6 @@ struct PlanArgs {
     // block kernel: the instances interleaved in one warp must agree on the workspace layout whatever their plans are ->
     // array strides of the LAUNCH (maxima over its plans): buses, value blocks
     int lay_nb, lay_nblkA;
-    const unsigned char *stage_src;   // block kernel with a TMA-staged plan: the plan's copy in global memory (streaming loads need it)
     // block kernel, staged launches: the static grid arrays the solve reads (line admittances, nominal voltages, unit limits, the
     // static injections, the thermal limits), packed into one blob that is staged next to the plan; nullptr: DevGrid's own
     // pointers (through L1 / L2 — cold after every L2 flush: ~15 dependent misses per warp in a one-wave launch)

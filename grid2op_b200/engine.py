@@ -108,6 +108,11 @@ def make_obs_desc(t: dict):
 
 
 def lib_path() -> str:
+    """The engine library: B200PF_LIB names another build of it (an instrumented copy, or an older build to compare
+    against); the default is the one build() leaves next to this file."""
+    p = os.environ.get("B200PF_LIB")
+    if p:
+        return os.path.abspath(p)
     return os.path.join(os.path.dirname(os.path.abspath(__file__)), "libb200pf.so")
 
 
