@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <unordered_map>
@@ -92,15 +93,14 @@ struct b200pf_handle {
     bool series_dev_topo_ahead = false;                     // the warp kernel tripped lines in d_series_topo on the device: the host mirror / plans lag
     bool series_plans_stale = false;                        // the cache was reset under the series' plan ids: re-resolve before the next step
     int64_t launches = 0;
-    int redo_pdl = 1;                                       // B200PF_REDO_PDL=0: plain stream-ordered launch of the safety net
     int redo_enabled = 1;                                   // pivoting re-solve of what the planned kernel leaves as ST_DIV (B200PF_NO_REDO=1 turns it off)
     int dbg_div_mod = 0;                                    // test knob, see b200pf_set_debug
-    int64_t redo_launches = 0;
-    int *series_flag = nullptr; int series_step_no = 0; int *d_ticket = nullptr; bool flag_in_redo = false;   // completion flag of series steps
-    // global-memory matrices of the safety net (large grids), one region per launching stream: chunk / group launches of one
-    // handle run concurrently, and two safety-net launches in flight must never share a CTA's matrix
-    struct RedoMat { unsigned char *d = nullptr; size_t stride = 0; int ctas = 0; };
-    std::unordered_map<cudaStream_t, RedoMat> redo_mats;
+    int *series_flag = nullptr; int series_step_no = 0;    // completion flag of series steps
+    // safety net, per launching stream (chunk / group launches of one handle run concurrently): the control word of its tail
+    // launch (one stream's armed re-solve must not stand in for another's), and on the large grids the global-memory matrices
+    // (two safety-net launches in flight must never share a CTA's matrix)
+    struct RedoStream { RedoCtl *ctl = nullptr; unsigned char *mat = nullptr; size_t stride = 0; int ctas = 0; };
+    std::unordered_map<cudaStream_t, RedoStream> redo_streams;
     bool on_side_stream = false;                            // a chunk / group launch is being issued (h->stream is swapped for it)
     cudaEvent_t inst_plan_ev = nullptr; bool inst_plan_pending = false;   // last H2D copy out of h_inst_plan
     int last_smem = 0, last_T = 0, last_grid = 0, last_block = 0;
@@ -291,8 +291,6 @@ extern "C" int b200pf_create(const b200pf_grid_desc *gd, int max_batch, int devi
         const char *bw = getenv("B200PF_BLOCK_WPC"), *bs = getenv("B200PF_BLOCK_STAGE");
         if (bw && (atoi(bw) == 1 || atoi(bw) == 2 || atoi(bw) == 4)) { h->blk_wpc = atoi(bw); h->blk_wpc_pinned = 1; }
         if (bs && (bs[0] == '0' || bs[0] == '1')) h->blk_stage = bs[0] - '0';
-        const char *rp = getenv("B200PF_REDO_PDL");
-        if (rp && rp[0] == '0') h->redo_pdl = 0;
         const char *nr = getenv("B200PF_NO_REDO");              // measurement only: planned kernel without its safety net
         if (nr && nr[0] == '1') h->redo_enabled = 0;
         const char *var = getenv("B200PF_SPARSE_T");            // tuning: threads per instance of the planned kernel
@@ -309,7 +307,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     for (void *p : h->dev_allocs) cudaFree(p);
     if (h->d_plan_blobs) cudaFree(h->d_plan_blobs);
     if (h->d_plan_off) cudaFree(h->d_plan_off);
-    for (auto &kv : h->redo_mats) if (kv.second.d) cudaFree(kv.second.d);
+    for (auto &kv : h->redo_streams) { if (kv.second.ctl) cudaFree(kv.second.ctl); if (kv.second.mat) cudaFree(kv.second.mat); }
     void *pinned[] = {h->h_topo, h->h_inj, h->h_out, h->h_status, h->h_iters, h->h_busv, h->h_rows, h->h_inst_plan};
     for (void *p : pinned) if (p) cudaFreeHost(p);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
@@ -675,7 +673,7 @@ static int plan_select(b200pf_handle *h, const int8_t *host_topo, int n_src, int
 }
 
 template <int T, int MINB, bool PROT = false>
-static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, int variant) {
+static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd, int variant) {
     const DevGrid &g = h->g;
     auto kern = pf_kernel_sparse<T, MINB, PROT>;
     const int smem = sel.smem;
@@ -705,7 +703,7 @@ static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &se
     const int rounds = (a.batch + resident - 1) / resident;
     int grid = (a.batch + rounds - 1) / rounds;
     if (grid < 1) grid = 1;
-    kern<<<grid, T, (size_t)smem, h->stream>>>(g, a, pa);
+    kern<<<grid, T, (size_t)smem, h->stream>>>(g, a, pa, rd);
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = T; h->last_kernel = 3;
@@ -716,22 +714,22 @@ static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &se
 // planned kernel: one warp per instance for the 5/14/36-substation grids, with as many one-warp CTAs per SM as the
 // workspace allows (up to the hardware's 32); two warps per instance for the large grids (118 substations, ~22 KB of
 // workspace per instance limit an SM to ~10 instances: the second warp doubles the warps in flight).
-static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel);
-static int launch_sparse(b200pf_handle *h, const RunArgs &a, const PlanSel &sel) {
-    if (h->blk) return launch_block(h, a, sel);
+static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd);
+static int launch_sparse(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd) {
+    if (h->blk) return launch_block(h, a, sel, rd);
     const int per_sm = h->max_smem_optin / (sel.smem + 1024);
     if (a.prot) {     // protections: one launch per cascade round, see series_step_planned_prot
-        if (h->plan_T == 128) return launch_sparse_t<128, 4, true>(h, a, sel, 14);
-        if (h->plan_T == 64) return launch_sparse_t<64, 10, true>(h, a, sel, 15);
-        return launch_sparse_t<32, 16, true>(h, a, sel, 13);
+        if (h->plan_T == 128) return launch_sparse_t<128, 4, true>(h, a, sel, rd, 14);
+        if (h->plan_T == 64) return launch_sparse_t<64, 10, true>(h, a, sel, rd, 15);
+        return launch_sparse_t<32, 16, true>(h, a, sel, rd, 13);
     }
-    if (h->plan_T == 128) return launch_sparse_t<128, 4>(h, a, sel, 4);
-    if (h->plan_T == 64) return launch_sparse_t<64, 10>(h, a, sel, 5);
-    if (per_sm >= 32 && h->sparse_minb == 28) return launch_sparse_t<32, 28>(h, a, sel, 7);   // 73 registers, 4144 resident warps
-    if (per_sm >= 32) return launch_sparse_t<32, 32>(h, a, sel, 1);
-    if (per_sm >= 24) return launch_sparse_t<32, 24>(h, a, sel, 2);
-    if (per_sm >= 16) return launch_sparse_t<32, 16>(h, a, sel, 3);
-    return launch_sparse_t<32, 8>(h, a, sel, 6);
+    if (h->plan_T == 128) return launch_sparse_t<128, 4>(h, a, sel, rd, 4);
+    if (h->plan_T == 64) return launch_sparse_t<64, 10>(h, a, sel, rd, 5);
+    if (per_sm >= 32 && h->sparse_minb == 28) return launch_sparse_t<32, 28>(h, a, sel, rd, 7);   // 73 registers, 4144 resident warps
+    if (per_sm >= 32) return launch_sparse_t<32, 32>(h, a, sel, rd, 1);
+    if (per_sm >= 24) return launch_sparse_t<32, 24>(h, a, sel, rd, 2);
+    if (per_sm >= 16) return launch_sparse_t<32, 16>(h, a, sel, rd, 3);
+    return launch_sparse_t<32, 8>(h, a, sel, rd, 6);
 }
 
 // Sizing of the generic pivoting kernel for nb_cap active buses: threads per instance, matrix bytes (see the policy above
@@ -759,42 +757,44 @@ static int generic_config(b200pf_handle *h, int cap, int jt, int *T_out, size_t 
     return 0;
 }
 
-// Safety net behind a planned launch (b200pf_redo.cuh): re-solves, with partial pivoting, the instances of the launch whose
-// status reads ST_DIV.  Same stream, no host round trip.  fp64 Jacobian whenever the actual systems fit the workspace with
-// it (5 / 14 / 36 substations), fp32 band LU otherwise (118 substations).
-template <int T, typename JT>
-static int launch_redo_t(b200pf_handle *h, const RunArgs &a, int max_ctas) {
+// Safety net of a planned launch (b200pf_redo.cuh): the configuration of the pivoting re-solve the planned kernel tail-launches
+// when one of its instances ends as ST_DIV (RedoDesc).  fp64 Jacobian whenever the actual systems fit the workspace with it
+// (5 / 14 / 36 substations), in global memory otherwise (118 substations).
+template <int T>
+static int redo_smem(b200pf_handle *h, const RedoDesc &rd, int *smem_out) {
     const DevGrid &g = h->g;
     // (matrix in global memory: the shared-memory workspace only holds the bus arrays)
-    WsLayout L = ws_layout(a.nb_cap, g.n_slot, g.n_line, g.n_inj, a.redo_mat ? (size_t)16 : (size_t)a.mat_bytes);
+    WsLayout L = ws_layout(rd.nb_cap, g.n_slot, g.n_line, g.n_inj, rd.mat ? (size_t)16 : (size_t)rd.mat_bytes);
     const size_t smem = L.total;
     if (smem > (size_t)h->max_smem_optin) return fail(B200PF_E_CAPACITY, "workspace does not fit in shared memory");
-    auto kern = pf_kernel_redo<T, JT>;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int grid = (a.batch + 31) / 32;
-    if (grid > max_ctas) grid = max_ctas;
-    if (grid < 1) grid = 1;
-    {   // programmatic dependent launch: the launch latency of this (almost always idle) kernel overlaps the planned kernel's tail
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)T); cfg.dynamicSmemBytes = smem; cfg.stream = h->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = h->redo_pdl ? 1 : 0;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        const int wsb = (int)smem;
-        CU(cudaLaunchKernelEx(&cfg, kern, g, a, wsb));
-        if (a.done_flag) h->flag_in_redo = true;
+    // The attribute holds for launches from the device as well.  It is set only when a launch needs more than any before it
+    // (per device and variant, shared by all handles: a larger limit never hurts): this runs ahead of every planned launch,
+    // and setting the attribute each time kept the GPU waiting for the host between steps.
+    static std::mutex mu;
+    static std::unordered_map<int, int> done;           // device * 1024 + T -> largest limit set
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        int &cur = done[h->device * 1024 + T];
+        if ((int)smem > cur) {
+            CU(cudaFuncSetAttribute(pf_kernel_redo<T, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            cur = (int)smem;
+        }
     }
-    CU(cudaGetLastError());
-    h->redo_launches++;
+    *smem_out = (int)smem;
     return 0;
 }
 
-static int launch_redo(b200pf_handle *h, RunArgs a, int nb_cap_req) {
+static int redo_config(b200pf_handle *h, const RunArgs &a, int nb_cap_req, RedoDesc *rd) {
+    *rd = RedoDesc{};
     if (!h->redo_enabled || a.is_dc || !a.topo) return 0;     // (the DC solve is a product with the plan's inverse: nothing to pivot)
     const DevGrid &g = h->g;
     int cap = nb_cap_req;
     if (cap <= 0 || cap > g.n_slot) cap = g.n_slot;
+    b200pf_handle::RedoStream &rs = h->redo_streams[h->stream];
+    if (!rs.ctl) {
+        CU(cudaMalloc(&rs.ctl, sizeof(RedoCtl)));
+        CU(cudaMemsetAsync(rs.ctl, 0, sizeof(RedoCtl), h->stream));
+    }
     // always an fp64 Jacobian with partial pivoting, like the reference's solver.  Where the worst-case system (every bus slot
     // active) fits the shared-memory workspace it lives there; on the large grids (118 substations: 472 x 474 x 8 B) every
     // CTA of the launch gets a matrix in global memory instead
@@ -803,19 +803,17 @@ static int launch_redo(b200pf_handle *h, RunArgs a, int nb_cap_req) {
     const size_t fixed = ws_fixed_bytes(cap, g.n_slot, g.n_line, g.n_inj);
     const size_t worst = ws_mat_worst(cap, 8);
     int max_ctas = h->sm_count * 8;
-    a.redo_mat = nullptr; a.redo_mat_stride = 0;
     if (fixed + worst > (size_t)h->max_smem_optin) {
         // (the handle's main stream gets one matrix per SM; the chunk / group streams a smaller set each: the path is rare)
         max_ctas = h->on_side_stream ? 32 : h->sm_count;
-        b200pf_handle::RedoMat &rm = h->redo_mats[h->stream];
-        if (!rm.d || rm.stride < worst || rm.ctas < max_ctas) {
+        if (!rs.mat || rs.stride < worst || rs.ctas < max_ctas) {
             CU(cudaStreamSynchronize(h->stream));
-            if (rm.d) CU(cudaFree(rm.d));
-            rm.d = nullptr;
-            CU(cudaMalloc(&rm.d, worst * (size_t)max_ctas));
-            rm.stride = worst; rm.ctas = max_ctas;
+            if (rs.mat) CU(cudaFree(rs.mat));
+            rs.mat = nullptr;
+            CU(cudaMalloc(&rs.mat, worst * (size_t)max_ctas));
+            rs.stride = worst; rs.ctas = max_ctas;
         }
-        a.redo_mat = rm.d; a.redo_mat_stride = rm.stride;
+        rd->mat = rs.mat; rd->mat_stride = rs.stride;
         want = worst;
         const size_t d = 2 * (size_t)cap;
         T = d <= 64 ? 32 : (d <= 128 ? 128 : (d <= 256 ? 256 : 512));
@@ -823,13 +821,20 @@ static int launch_redo(b200pf_handle *h, RunArgs a, int nb_cap_req) {
         int rc = generic_config(h, cap, 8, &T, &want);
         if (rc) return rc;
     }
-    a.redo = 1; a.nb_cap = cap; a.mat_bytes = (int)want;
+    rd->T = T; rd->nb_cap = cap; rd->mat_bytes = (int)want; rd->ctl = rs.ctl;
+    rd->grid = (a.batch + 31) / 32;
+    if (rd->grid > max_ctas) rd->grid = max_ctas;
+    if (rd->grid < 1) rd->grid = 1;
+    int rc;
     switch (T) {
-        case 32: return launch_redo_t<32, double>(h, a, max_ctas);
-        case 128: return launch_redo_t<128, double>(h, a, max_ctas);
-        case 256: return launch_redo_t<256, double>(h, a, max_ctas);
-        default: return launch_redo_t<512, double>(h, a, max_ctas);
+        case 32: rc = redo_smem<32>(h, *rd, &rd->smem); break;
+        case 128: rc = redo_smem<128>(h, *rd, &rd->smem); break;
+        case 256: rc = redo_smem<256>(h, *rd, &rd->smem); break;
+        default: rc = redo_smem<512>(h, *rd, &rd->smem); break;
     }
+    if (rc) return rc;
+    rd->on = 1;
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -866,7 +871,7 @@ static int stat_sync(b200pf_handle *h) {
 }
 
 template <int T, int U, int MINB, bool PROT, int WPC = 1, bool STAGE = false, bool UNI = false, int MODE = 0>
-static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel) {
+static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd) {
     const DevGrid &g = h->g;
     constexpr int G = T < 32 ? 32 / T : 1;
     constexpr int BLOCK = (T < 32 ? 32 : T) * WPC;
@@ -911,7 +916,7 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     const int rounds = (n_cta_work + resident - 1) / resident;
     int grid = (n_cta_work + rounds - 1) / rounds;
     if (grid < 1) grid = 1;
-    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(g, a, pa, ws, plan_bytes, plan_src, row_ahead);
+    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(g, a, pa, ws, plan_bytes, plan_src, row_ahead, rd);
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 4;
@@ -928,7 +933,7 @@ static bool block_variant_exists(int T, int U) {
     return false;
 }
 
-static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel) {
+static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd) {
     const int T = h->blk_T, U = h->blk_U;
     // Shared-plan launches of the default (8 x 1) variant: CTAs of WPC warps that fetch the plan ONCE into shared memory with a bulk
     // asynchronous copy (TMA) and run in lockstep (DESIGN.md 4.2).  Knobs to compare: B200PF_BLOCK_STAGE=0 (plan through L1), B200PF_BLOCK_WPC=1/2/4, B200PF_BLOCK_UNI=0.
@@ -938,28 +943,28 @@ static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel) 
             // warps per CTA: 2 up to 32 k instances (finer SM balance: 167 vs 158 M/s at batch 16 384), 4 beyond (197 vs 189 M/s at
             // 65 536: one staged copy serves more instances); B200PF_BLOCK_WPC pins it
             const int wpc = h->blk_wpc_pinned ? h->blk_wpc : (a.batch <= 32768 ? 2 : 4);
-            if (wpc == 1) return launch_block_t<8, 1, 16, false, 1, true, true>(h, a, sel);
+            if (wpc == 1) return launch_block_t<8, 1, 16, false, 1, true, true>(h, a, sel, rd);
             // the stepping paths (AC, inputs = chronics rows) run the variant specialised for exactly that
             const bool ac_rows = !a.is_dc && a.series && h->blk_spec;
-            if (wpc == 2) return ac_rows ? launch_block_t<8, 1, 8, false, 2, true, true, 1>(h, a, sel) : launch_block_t<8, 1, 8, false, 2, true, true>(h, a, sel);
-            return ac_rows ? launch_block_t<8, 1, 4, false, 4, true, true, 1>(h, a, sel) : launch_block_t<8, 1, 4, false, 4, true, true>(h, a, sel);
+            if (wpc == 2) return ac_rows ? launch_block_t<8, 1, 8, false, 2, true, true, 1>(h, a, sel, rd) : launch_block_t<8, 1, 8, false, 2, true, true>(h, a, sel, rd);
+            return ac_rows ? launch_block_t<8, 1, 4, false, 4, true, true, 1>(h, a, sel, rd) : launch_block_t<8, 1, 4, false, 4, true, true>(h, a, sel, rd);
         }
-        return launch_block_t<8, 1, 4, false, 4, true, false>(h, a, sel);
+        return launch_block_t<8, 1, 4, false, 4, true, false>(h, a, sel, rd);
     }
-    if (!a.prot && T == 8 && U == 1 && h->blk_wpc == 4 && h->blk_wpc_pinned && !h->blk_stage) return launch_block_t<8, 1, 4, false, 4, false, false>(h, a, sel);
+    if (!a.prot && T == 8 && U == 1 && h->blk_wpc == 4 && h->blk_wpc_pinned && !h->blk_stage) return launch_block_t<8, 1, 4, false, 4, false, false>(h, a, sel, rd);
     if (!a.prot && T == 8 && U == 1) {
         // lockstep warps (one plan for the whole launch, whole warps): full-mask barriers / votes instead of per-instance collectives
         const bool uni = h->blk_uni && !sel.d_inst_plan && a.batch % 4 == 0;
         // register budget: 16 warps x 128 registers per SM
-        if (uni) return launch_block_t<8, 1, 16, false, 1, false, true>(h, a, sel);
-        return launch_block_t<8, 1, 16, false>(h, a, sel);
+        if (uni) return launch_block_t<8, 1, 16, false, 1, false, true>(h, a, sel, rd);
+        return launch_block_t<8, 1, 16, false>(h, a, sel, rd);
     }
     if (a.prot) {
-#define X(t, u) if (T == t && U == u) return launch_block_t<t, u, (t <= 32 ? 8 : 4), true>(h, a, sel);
+#define X(t, u) if (T == t && U == u) return launch_block_t<t, u, (t <= 32 ? 8 : 4), true>(h, a, sel, rd);
         B200PF_BLOCK_VARIANTS(X)
 #undef X
     } else {
-#define X(t, u) if (T == t && U == u) return launch_block_t<t, u, (t <= 32 ? 8 : 4), false>(h, a, sel);
+#define X(t, u) if (T == t && U == u) return launch_block_t<t, u, (t <= 32 ? 8 : 4), false>(h, a, sel, rd);
         B200PF_BLOCK_VARIANTS(X)
 #undef X
     }
@@ -968,9 +973,9 @@ static int launch_block(b200pf_handle *h, const RunArgs &a, const PlanSel &sel) 
 
 static int launch(b200pf_handle *h, RunArgs a, int nb_cap_req, const PlanSel *sel = nullptr) {
     if (sel) {
-        int rc = launch_sparse(h, a, *sel);
-        if (rc || a.prot) return rc;           // (protections: series_step_planned_prot launches the safety net itself)
-        return launch_redo(h, a, nb_cap_req);
+        RedoDesc rd;
+        int rc = redo_config(h, a, nb_cap_req, &rd);
+        return rc ? rc : launch_sparse(h, a, *sel, rd);
     }
     const DevGrid &g = h->g;
     if (h->env_flags < 0) {
@@ -1184,9 +1189,9 @@ static int series_step_planned_prot(b200pf_handle *h, RunArgs a) {
         PlanSel sel;
         sel.single = 0; sel.d_inst_plan = h->d_series_plan;
         sel_layout(h, &sel, false);
-        int rc = launch_sparse(h, a, sel);
-        if (rc) return rc;
-        if ((rc = launch_redo(h, a, 0))) return rc;       // pivoting re-solve (+ the protection rules) of what ended as ST_DIV
+        RedoDesc rd;       // (the re-solve applies the protection rules to what it solves)
+        int rc = redo_config(h, a, 0, &rd);
+        if (rc || (rc = launch_sparse(h, a, sel, rd))) return rc;
         int nflag = 0;
         CU(cudaMemcpyAsync(&nflag, h->d_nflag, 4, cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));
@@ -1224,11 +1229,10 @@ extern "C" int b200pf_series_step(b200pf_handle *h, int is_dc, int max_iter, dou
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
     CU(cudaSetDevice(h->device));
-    h->flag_in_redo = false;
     if (h->series_flag) h->series_step_no++;
     int rc = series_step_impl(h, is_dc, max_iter, tol_mva, nb_cap);
     if (rc) return rc;
-    if (h->series_flag && !h->flag_in_redo) {        // no safety-net launch carried the flag: publish it with a one-thread kernel
+    if (h->series_flag) {
         pf_kernel_flag<<<1, 1, 0, h->stream>>>(h->series_flag, h->series_step_no);
         CU(cudaGetLastError());
     }
@@ -1238,7 +1242,6 @@ extern "C" int b200pf_series_step(b200pf_handle *h, int is_dc, int max_iter, dou
 extern "C" int b200pf_series_bind_flag(b200pf_handle *h, int32_t *d_flag) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     CU(cudaSetDevice(h->device));
-    if (!h->d_ticket) { CU(cudaMalloc(&h->d_ticket, 16)); h->dev_allocs.push_back(h->d_ticket); CU(cudaMemsetAsync(h->d_ticket, 0, 16, h->stream)); }
     h->series_flag = d_flag; h->series_step_no = 0;
     return 0;
 }
@@ -1249,7 +1252,6 @@ static int series_step_impl(b200pf_handle *h, int is_dc, int max_iter, double to
     a.iters = h->x_iters ? h->x_iters : h->d_iters; a.busv = nullptr;
     a.series = 1; a.chron = h->d_chron; a.n_scen = h->n_scen; a.n_rows = h->n_rows; a.scen = h->d_scen; a.t = h->d_t;
     a.static_inj = h->d_static_inj; a.th_lim = h->d_thlim; a.rho = h->x_rho ? h->x_rho : h->d_rho;
-    if (h->series_flag && !h->prot) { a.done_flag = h->series_flag; a.done_value = h->series_step_no; a.done_ticket = h->d_ticket; }
     if (h->prot) {
         a.prot = 1; a.from_reset = h->next_reset; a.max_pc = h->max_pc; a.hard_thr = h->hard_thr; a.soft_thr = h->soft_thr;
         a.pcount = h->d_pcount; a.ts_over = h->d_tsover; a.disc = h->d_disc; a.done = h->d_done;
@@ -1674,7 +1676,18 @@ extern "C" int b200pf_set_debug(b200pf_handle *h, int planned_div_mod, int redo_
     return 0;
 }
 
-extern "C" int64_t b200pf_redo_launch_count(const b200pf_handle *h) { return h ? h->redo_launches : 0; }
+// the planned kernels count their tail launches in the control words: waits for the device, then reads them
+extern "C" int64_t b200pf_redo_launch_count(const b200pf_handle *h) {
+    if (!h || cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return 0;
+    int64_t n = 0;
+    for (const auto &kv : h->redo_streams) {
+        RedoCtl c{};
+        if (!kv.second.ctl) continue;
+        if (cudaMemcpy(&c, kv.second.ctl, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
+        n += c.launches;
+    }
+    return n;
+}
 
 extern "C" int b200pf_plan_counters(const b200pf_handle *h, int64_t *out4) {
     if (!h || !out4) return fail(B200PF_E_ARG, "null pointer");

@@ -15,8 +15,8 @@
 //     eight scalar operations of the old stream; pivot rows are normalised with the explicit 2x2 inverse (which pivots
 //     inside the block), U operations per lane and row are loaded before any is stored (ILP inside a pass).
 // Arithmetic plan unchanged: fp64 state / mismatch / flows, fp32 Jacobian and solve, the fp64 residual decides convergence
-// with pandapower's criterion; same result record, same status classes.  ST_DIV is never final: pf_kernel_redo
-// (b200pf_redo.cuh) re-solves such instances with partial pivoting behind every launch.
+// with pandapower's criterion; same result record, same status classes.  ST_DIV is never final: the first such instance
+// makes the kernel tail-launch pf_kernel_redo (b200pf_redo.cuh), which re-solves them with partial pivoting.
 // With B200PF_EMULATE the same source compiles as plain host C++ (a phase = a loop over the lanes of ONE instance, the
 // instances of a warp one after the other on the same interleaved workspace): tests/ use that build on machines without a GPU.
 #pragma once
@@ -132,7 +132,8 @@ PF_DEV size_t block_srow_off(int Lnb, int LnblkA, int nsh, int nl) {
 // STAGE: the plan (and pa.stat) are the launch's copies in shared memory, and the kernel has already run block_row /
 // block_row_copy for this instance (for its first instance group while the plan's bulk copy was in flight).
 template <int T, int U, int G, bool PROT, bool UNI = false, int MODE = 0, bool STAGE = false>
-PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int gi, int tid0, unsigned imask) {
+PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int gi, int tid0, unsigned imask,
+                        const RedoDesc &rd = RedoDesc()) {
 #ifndef B200PF_EMULATE
     const int tid = tid0;
 #endif
@@ -515,7 +516,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         const double *qmins = F64(o_qmins), *qmaxs = F64(o_qmaxs);
         PF_PHASE {
           if (UNI && fstat >= 0) {                             // lockstep: the failure record, stored without leaving the warp
-            if (tid == 0) { a.status[inst] = fstat; a.iters[inst] = fiters; }
+            if (tid == 0) { a.status[inst] = fstat; a.iters[inst] = fiters; if (fstat == ST_DIV) PF_REDO_ARM(g, a, rd); }
             if (out) for (int k = tid; k < g.n_out; k += T) out[k] = PF_QNANF();
             if (a.busv) for (int k = tid; k < 2 * g.n_slot; k += T) a.busv[(size_t)inst * 2 * g.n_slot + k] = PF_QNAN();
             if (a.rho) for (int k = tid; k < g.n_line; k += T) a.rho[(size_t)inst * g.n_line + k] = PF_QNANF();
@@ -706,11 +707,8 @@ __device__ __forceinline__ void pb_stage_wait(uint64_t *mbar) {
 template <int T, int U, int MINB, bool PROT, int WPC = 1, bool STAGE = false, bool UNI = false, int MODE = 0>
 __global__ void __launch_bounds__((T < 32 ? 32 : T) * WPC, MINB)
 pf_kernel_block(const DevGrid g, const RunArgs a, const PlanArgs pa_in, const int ws_bytes, const int plan_bytes, const unsigned char *plan_src,
-                const int row_ahead) {
+                const int row_ahead, const RedoDesc rd) {
     extern __shared__ __align__(16) unsigned char smem[];
-    // the safety-net kernel behind this launch (programmatic dependent launch) may be set up right away: it parks at its
-    // griddepcontrol.wait until this grid has completed, so its launch latency is off the critical path
-    asm volatile("griddepcontrol.launch_dependents;");
 #if PB_CLOCK_ON
     const bool clk_lane0 = (threadIdx.x & 31) == 0;
     const long long clk_entry = clock64();
@@ -763,7 +761,10 @@ pf_kernel_block(const DevGrid g, const RunArgs a, const PlanArgs pa_in, const in
         if (k < a.batch) {
             const int inst = (PROT && a.inst_list) ? a.inst_list[k] : k;
             if (STAGE && !first) load_rows(inst);
-            solve_block<T, U, G, PROT, UNI, MODE, STAGE>(g, a, pa, inst, ws, gi, j, imask);
+            solve_block<T, U, G, PROT, UNI, MODE, STAGE>(g, a, pa, inst, ws, gi, j, imask, rd);
+            // free-running instances leave solve_block at their failure (block_fail); the safety net is armed here, once per
+            // instance, outside the diverged code (lockstep warps arm it in solve_block's failure record)
+            if (!UNI && rd.on && j == 0 && a.status[inst] == ST_DIV) redo_arm(g, a, rd);
         }
         if (T <= 32) __syncwarp(); else __syncthreads();
     }

@@ -85,9 +85,6 @@ struct RunArgs {
     int redo;
     unsigned char *redo_mat;  // safety net on large grids: per-CTA matrix region in GLOBAL memory (an fp64 Jacobian of the 118-substation
     size_t redo_mat_stride;   // grid does not fit on chip; the path is rare, its speed does not matter), nullptr = shared memory
-    // completion flag of a series step (multi-GPU result collection without a collective): when the step's kernels are through,
-    // done_value is stored to *done_flag (may live in another GPU's memory); ticket: CTA counter of the writing kernel
-    int *done_flag; int done_value; int *done_ticket;
     int dbg_div_mod;         // test knob: > 0 makes the planned kernel give up (ST_DIV) on every instance with inst % mod == 0
 };
 

@@ -7,11 +7,12 @@
 // fp64 Jacobian where the workspace allows it) before the status leaves the library, so that `runpf -> (False, exc)`
 // (pPB:1241-1255) is only ever reported for states the pivoting solver gives up on as well.
 //
-// One launch right behind the planned one, on the same stream, no host round trip: every CTA scans the status words of
-// 32 instances (one coalesced load), and re-solves those that read ST_DIV.  In the common case (no such instance) the
-// launch costs one load per CTA.
+// The planned kernel launches it itself, as a tail launch, the first time one of its instances ends as ST_DIV (redo_arm,
+// b200pf_sparse.cuh): it runs once the planned grid has completed, on the same stream, no host round trip, and a planned
+// launch without such an instance costs nothing here.  Every CTA scans the status words of 32 instances (one coalesced
+// load) and re-solves those that read ST_DIV.
 #pragma once
-#include "b200pf_kernel.cuh"
+#include "b200pf_sparse.cuh"
 
 namespace b200pf {
 
@@ -54,13 +55,11 @@ __device__ void redo_prot_round(const DevGrid &g, const RunArgs &a, int inst, in
 
 template <int T, typename JT>
 __global__ void __launch_bounds__(T, (T == 32) ? 8 : 1)
-pf_kernel_redo(const DevGrid g, const RunArgs a, const int ws_bytes) {
+pf_kernel_redo(const DevGrid g, const RunArgs a, RedoCtl *ctl) {
     extern __shared__ __align__(16) unsigned char smem[];
-    (void)ws_bytes;
     const int tid = threadIdx.x;
-    // launched with programmatic stream serialisation right behind the planned kernel: this grid is set up while that one
-    // drains, and waits here until it has completed and its results are visible
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    // no CTA of the planned grid that launched this one runs any more: the next planned launch on this stream may arm again
+    if (blockIdx.x == 0 && tid == 0) ctl->armed = 0;
     for (int first = blockIdx.x * 32; first < a.batch; first += gridDim.x * 32) {
         // every warp of the CTA computes the same mask (the status words are only written at the very end of a
         // re-solve, behind group barriers that all warps pass)
@@ -83,20 +82,6 @@ pf_kernel_redo(const DevGrid g, const RunArgs a, const int ws_bytes) {
             gsync<T>();
         }
     }
-    if (a.done_flag) {
-        // the step is complete when the LAST CTA of this (last) kernel of the step is: it publishes the step number, system-wide
-        // (the flag may sit in the agent rank's HBM, next to the results the planned kernel stored there)
-        __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            const int t = atomicAdd(a.done_ticket, 1);
-            if (t == (int)gridDim.x - 1) {
-                *a.done_ticket = 0;
-                __threadfence_system();
-                *reinterpret_cast<volatile int *>(a.done_flag) = a.done_value;
-            }
-        }
-    }
 }
 
 // env.reset() of single instances of a bound series: counters, flags and the row pointer back to a fresh episode
@@ -112,9 +97,10 @@ __global__ void pf_kernel_series_reset(int n, const int *idx, const int *t_new, 
     }
 }
 
-// paths without a safety-net launch: one thread publishes the step number behind the step's kernels
+// completion flag of a series step (multi-GPU result collection without a collective): one thread publishes the step number,
+// system-wide (the flag may sit in the agent rank's HBM, next to the results the step stored there).  Stream order puts it
+// behind the step's kernels, the safety net they tail-launched included.
 __global__ void pf_kernel_flag(int *flag, int value) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
     __threadfence_system();
     *reinterpret_cast<volatile int *>(flag) = value;
 }

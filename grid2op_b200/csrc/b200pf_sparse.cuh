@@ -12,8 +12,8 @@
 // Same arithmetic plan as the other kernels (fp64 state / mismatch / flows, fp32 Jacobian and solve, the fp64
 // residual decides convergence with pandapower's criterion), same result record, same status classes.
 // Elimination is WITHOUT pivoting on the (theta_i, |V|_i)-interleaved minimum-degree order: a breakdown shows
-// up as a non-finite update and ends as ST_DIV.  ST_DIV is never final here: the library launches pf_kernel_redo
-// (b200pf_redo.cuh) right behind this kernel, which re-solves every such instance with partial pivoting.
+// up as a non-finite update and ends as ST_DIV.  ST_DIV is never final here: the first such instance makes this kernel
+// tail-launch pf_kernel_redo (b200pf_redo.cuh), which re-solves every such instance with partial pivoting.
 //
 // The body is written as a sequence of PHASES separated by group barriers, every piece of state that crosses a
 // phase lives in the (shared-memory) workspace.  With B200PF_EMULATE the same source compiles as plain host
@@ -101,7 +101,6 @@ struct RunArgs {
     int *n_flag, *flag_list;
     int redo, dbg_div_mod;
     unsigned char *redo_mat; size_t redo_mat_stride;
-    int *done_flag; int done_value; int *done_ticket;
 };
 enum { ST_OK = 0, ST_DIV = 1, ST_UNSUP = 2, ST_NOREF = 3, ST_LARGE = 4, ST_DONE = 5 };
 enum { BT_PQ = 1, BT_PV = 2, BT_REF = 3 };
@@ -126,14 +125,57 @@ struct PlanArgs {
                          sh_vn, sh_vratio, static_inj, th_lim, total; } so;
 };
 
+// Safety net of the planned kernels (b200pf_redo.cuh).  The first instance of a planned launch that ends as ST_DIV makes
+// the kernel itself launch the pivoting re-solve, as a tail launch of its grid: it starts once the planned grid has completed,
+// and stream order counts the planned launch as complete only once the re-solve is.  A launch without such an instance
+// launches nothing.
+struct RedoCtl {              // one per stream of a handle, in device memory
+    int armed;                // 1: this stream's running planned launch has queued its re-solve (pf_kernel_redo clears it)
+    int launches;             // re-solves launched so far
+};
+struct RedoDesc {
+    int on;                   // 0: no safety net behind this launch (B200PF_NO_REDO, b200pf_set_debug, DC solves)
+    int T, grid, smem;        // pf_kernel_redo<T, double>: threads per instance, CTAs, dynamic shared memory
+    int nb_cap, mat_bytes;    // the re-solve's RunArgs: the planned launch's, with redo = 1 and these
+    unsigned char *mat; size_t mat_stride;      // -> RunArgs::redo_mat / redo_mat_stride
+    RedoCtl *ctl;
+};
+
+#ifdef B200PF_EMULATE
+#define PF_REDO_ARM(g, a, rd) ((void)(rd))
+#else
+template <int T, typename JT> __global__ void pf_kernel_redo(const DevGrid g, const RunArgs a, RedoCtl *ctl);
+// Called by one lane of every instance a planned kernel ends as ST_DIV: the first one of the launch tail-launches the re-solve
+// for the whole launch (pf_kernel_redo scans every status word of the launch).
+__device__ __forceinline__ void redo_arm(const DevGrid &g, const RunArgs &a, const RedoDesc &rd) {
+    if (!rd.on || atomicCAS(&rd.ctl->armed, 0, 1) != 0) return;
+    RunArgs r = a;
+    r.redo = 1; r.nb_cap = rd.nb_cap; r.mat_bytes = rd.mat_bytes; r.redo_mat = rd.mat; r.redo_mat_stride = rd.mat_stride;
+    // (one launch site: the parameter block is written once, whichever of the four variants runs)
+    void (*kern)(const DevGrid, const RunArgs, RedoCtl *);
+    switch (rd.T) {
+        case 32: kern = pf_kernel_redo<32, double>; break;
+        case 128: kern = pf_kernel_redo<128, double>; break;
+        case 256: kern = pf_kernel_redo<256, double>; break;
+        default: kern = pf_kernel_redo<512, double>; break;
+    }
+    kern<<<rd.grid, rd.T, rd.smem, cudaStreamTailLaunch>>>(g, r, rd.ctl);
+    atomicAdd(&rd.ctl->launches, 1);
+}
+#define PF_REDO_ARM(g, a, rd) redo_arm((g), (a), (rd))
+#endif
+
 template <int T>
-PF_DEV void sparse_fail(const DevGrid &g, const RunArgs &a, int inst, int status, int iters, int tid0) {
+PF_DEV void sparse_fail(const DevGrid &g, const RunArgs &a, int inst, int status, int iters, int tid0, const RedoDesc &rd) {
 #ifndef B200PF_EMULATE
     const int tid = tid0;
 #endif
     float *out = a.out ? a.out + (size_t)inst * g.n_out : nullptr;
     PF_PHASE {
-        if (tid == 0) { a.status[inst] = status; a.iters[inst] = iters; if (a.prot && a.done) a.done[inst] = 1; }
+        if (tid == 0) {
+            a.status[inst] = status; a.iters[inst] = iters; if (a.prot && a.done) a.done[inst] = 1;
+            if (status == ST_DIV) PF_REDO_ARM(g, a, rd);
+        }
         if (a.prot && a.disc && status == ST_DONE) for (int k = tid; k < g.n_line; k += T) a.disc[(size_t)inst * g.n_line + k] = -1;
         if (out) for (int k = tid; k < g.n_out; k += T) out[k] = PF_QNANF();
         if (a.busv) for (int k = tid; k < 2 * g.n_slot; k += T) a.busv[(size_t)inst * 2 * g.n_slot + k] = PF_QNAN();
@@ -144,7 +186,8 @@ PF_DEV void sparse_fail(const DevGrid &g, const RunArgs &a, int inst, int status
 }
 
 template <int T, bool PROT>
-PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int tid0) {
+PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, int inst, unsigned char *sm, int tid0,
+                         const RedoDesc &rd = RedoDesc()) {
 #ifndef B200PF_EMULATE
     const int tid = tid0;
 #endif
@@ -159,9 +202,9 @@ PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa,
         if (PROT && a.casc > 0) trow = trow == 0 ? a.n_rows - 1 : trow - 1;       // later cascade rounds re-solve the SAME row
         PF_PHASE { if (tid == 0 && a.n1_lines <= 0 && !(PROT && a.casc > 0)) a.t[inst] = (trow + 1 >= a.n_rows) ? 0 : trow + 1; }
     }
-    if (PROT && a.done[inst] && a.casc == 0) { sparse_fail<T>(g, a, inst, ST_DONE, 0, tid0); return; }
-    if (H.status != PLAN_ST_OK) { sparse_fail<T>(g, a, inst, H.status, 0, tid0); return; }
-    if (a.dbg_div_mod > 0 && inst % a.dbg_div_mod == 0) { sparse_fail<T>(g, a, inst, ST_DIV, 0, tid0); return; }   // test knob (b200pf_set_debug)
+    if (PROT && a.done[inst] && a.casc == 0) { sparse_fail<T>(g, a, inst, ST_DONE, 0, tid0, rd); return; }
+    if (H.status != PLAN_ST_OK) { sparse_fail<T>(g, a, inst, H.status, 0, tid0, rd); return; }
+    if (a.dbg_div_mod > 0 && inst % a.dbg_div_mod == 0) { sparse_fail<T>(g, a, inst, ST_DIV, 0, tid0, rd); return; }   // test knob (b200pf_set_debug)
     const int nb = H.nb, nl = g.n_line, nu = g.n_unit, nh = g.n_hidden, ng = g.n_gen, nld = g.n_load, nst = g.n_sto, nsh = g.n_shunt;
     const int d = H.d, nnzF = H.nnzF, nA = H.nA;
     const double base = g.base_mva;
@@ -257,7 +300,7 @@ PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa,
             }
         }
         bad = PF_ANY(bad);
-        if (bad) { sparse_fail<T>(g, a, inst, ST_DIV, 0, tid0); return; }
+        if (bad) { sparse_fail<T>(g, a, inst, ST_DIV, 0, tid0, rd); return; }
     }
     // ---- 3. Newton-Raphson ---------------------------------------------------------------------------------
     // Four phases per iteration: [lane = line: branch currents + off-diagonal Jacobian terms] [lane = bus: S(V), mismatch,
@@ -417,7 +460,7 @@ PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa,
             PF_SYNC();
         }
 #undef PF_OFFDIAG
-        if (!conv) { sparse_fail<T>(g, a, inst, ST_DIV, iters, tid0); return; }
+        if (!conv) { sparse_fail<T>(g, a, inst, ST_DIV, iters, tid0, rd); return; }
     } else {
         // DC: line lanes compute flows from the angles, bus lanes sum them for the slack share
         PF_PHASE {
@@ -594,12 +637,11 @@ PF_DEV void solve_sparse(const DevGrid &g, const RunArgs &a, const PlanArgs &pa,
 #ifndef B200PF_EMULATE
 template <int T, int MINB, bool PROT>
 __global__ void __launch_bounds__(T, MINB)
-pf_kernel_sparse(const DevGrid g, const RunArgs a, const PlanArgs pa) {
+pf_kernel_sparse(const DevGrid g, const RunArgs a, const PlanArgs pa, const RedoDesc rd) {
     extern __shared__ __align__(16) unsigned char smem[];
-    asm volatile("griddepcontrol.launch_dependents;");      // (the safety-net kernel behind this launch may be set up right away)
     for (int k = blockIdx.x; k < a.batch; k += gridDim.x) {
         const int inst = (PROT && a.inst_list) ? a.inst_list[k] : k;
-        solve_sparse<T, PROT>(g, a, pa, inst, smem, threadIdx.x);
+        solve_sparse<T, PROT>(g, a, pa, inst, smem, threadIdx.x, rd);
         sp_sync<T>();
     }
 }

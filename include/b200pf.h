@@ -282,12 +282,13 @@ int b200pf_ipc_close(void *d_ptr);
 
 /* Safety net of the planned kernel.  The planned kernel eliminates without pivoting on an fp32 Jacobian; the reference's
  * solver (pp.runpp, pPB:1097-1105) pivots in fp64, and a failed power flow is a game over (pPB:1241-1255,
- * grid2op/Environment/baseEnv.py:3523-3524).  Every planned launch is therefore followed, on the same stream and inside the
- * same C-ABI call, by a launch that re-solves with partial pivoting (fp64 Jacobian where the workspace allows) the instances
- * the planned kernel left as DIVERGED; a status only leaves the library after that.  b200pf_set_debug is a TEST knob:
+ * grid2op/Environment/baseEnv.py:3523-3524).  A planned launch that leaves an instance as DIVERGED therefore launches, from
+ * the device, on the same stream and inside the same C-ABI call, a re-solve with partial pivoting (fp64 Jacobian where the
+ * workspace allows) of every such instance; a status only leaves the library after that.  b200pf_set_debug is a TEST knob:
  * planned_div_mod > 0 makes the planned kernel give up on every instance with (index % planned_div_mod == 0), which
  * exercises the re-solve path; redo_enabled = 0 switches the safety net off (measurements).  Env B200PF_NO_REDO=1 presets
- * the latter.  b200pf_redo_launch_count: safety-net launches so far (they are not part of b200pf_launch_count). */
+ * the latter.  b200pf_redo_launch_count: safety-net launches so far (they are not part of b200pf_launch_count); it waits
+ * for the device, so read it after a fetch, not between the launches of a step. */
 int b200pf_set_debug(b200pf_handle *h, int planned_div_mod, int redo_enabled);
 int64_t b200pf_redo_launch_count(const b200pf_handle *h);
 
