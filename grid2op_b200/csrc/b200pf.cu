@@ -104,6 +104,7 @@ struct b200pf_handle {
     bool on_side_stream = false;                            // a chunk / group launch is being issued (h->stream is swapped for it)
     cudaEvent_t inst_plan_ev = nullptr; bool inst_plan_pending = false;   // last H2D copy out of h_inst_plan
     int last_smem = 0, last_T = 0, last_grid = 0, last_block = 0;
+    int last_cfg[8] = {-1, -1, -1, -1, -1, -1, -1, -1};    // template parameters of the last launch (b200pf_last_launch_config)
     // observation layer (b200pf_obs_bind / b200pf_observe)
     ObsArgs obs{}; int obs_batch = 0, obs_rows = 0;
     std::vector<void *> obs_allocs;
@@ -371,6 +372,13 @@ extern "C" int b200pf_grid_max_active_buses(const b200pf_grid_desc *gd, int n, c
 // ------------------------------------------------------------------------------------------------
 // launch configuration
 // ------------------------------------------------------------------------------------------------
+// template parameters of the launch just issued, in the order of b200pf_last_launch_config (missing ones: -1)
+static void set_last_cfg(b200pf_handle *h, std::initializer_list<int> cfg) {
+    int k = 0;
+    for (int v : cfg) h->last_cfg[k++] = v;
+    for (; k < 8; ++k) h->last_cfg[k] = -1;
+}
+
 template <int T, typename JT>
 static int launch_t(b200pf_handle *h, const RunArgs &a) {
     const DevGrid &g = h->g;
@@ -397,6 +405,7 @@ static int launch_t(b200pf_handle *h, const RunArgs &a) {
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = (int)smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 2;
+    set_last_cfg(h, {});
     return 0;
 }
 
@@ -424,6 +433,7 @@ static int launch_small(b200pf_handle *h, RunArgs a, int cap) {
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = L.total; h->last_T = 32; h->last_grid = grid; h->last_block = 32; h->last_kernel = 1;
+    set_last_cfg(h, {});
     (void)g;
     return 0;
 }
@@ -707,6 +717,7 @@ static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &se
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = T; h->last_kernel = 3;
+    set_last_cfg(h, {T, -1, MINB, PROT ? 1 : 0});
     return 0;
 }
 
@@ -920,6 +931,7 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     CU(cudaGetLastError());
     h->launches++;
     h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 4;
+    set_last_cfg(h, {T, U, MINB, PROT ? 1 : 0, WPC, STAGE ? 1 : 0, UNI ? 1 : 0, MODE});
     return 0;
 }
 
@@ -1811,5 +1823,10 @@ extern "C" int b200pf_last_launch_info(const b200pf_handle *h, int *smem_bytes, 
     if (threads_per_instance) *threads_per_instance = h->last_T;
     if (grid_blocks) *grid_blocks = h->last_grid;
     if (block_threads) *block_threads = h->last_block;
+    return 0;
+}
+extern "C" int b200pf_last_launch_config(const b200pf_handle *h, int *cfg8) {
+    if (!h || !cfg8) return fail(B200PF_E_ARG, "null pointer");
+    for (int k = 0; k < 8; ++k) cfg8[k] = h->last_cfg[k];
     return 0;
 }

@@ -37,6 +37,7 @@ ABI_SYMBOLS = (
     "b200pf_set_debug", "b200pf_redo_launch_count",
     "b200pf_device_alloc", "b200pf_device_free", "b200pf_ipc_export", "b200pf_ipc_open", "b200pf_ipc_close", "b200pf_device_read", "b200pf_plan_counters", "b200pf_series_bind_flag",
     "b200pf_series_reset_instances", "b200pf_grid_max_active_buses", "b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats",
+    "b200pf_last_launch_config",
 )
 
 
@@ -169,6 +170,7 @@ def load_library():
     lib.b200pf_launch_count.argtypes = [vp]
     lib.b200pf_launch_count.restype = C.c_int64
     lib.b200pf_last_launch_info.argtypes = [vp] + [C.POINTER(i32)] * 4
+    lib.b200pf_last_launch_config.argtypes = [vp, C.POINTER(i32)]
     lib.b200pf_set_kernel_policy.argtypes = [vp, i32]
     lib.b200pf_plan_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(i32)]
     lib.b200pf_set_debug.argtypes = [vp, i32, i32]
@@ -198,7 +200,7 @@ def load_library():
     lib.b200pf_redo_launch_count.restype = C.c_int64
     for nm in ("b200pf_create", "b200pf_destroy", "b200pf_sizes", "b200pf_run_host", "b200pf_run_device",
                "b200pf_series_bind", "b200pf_series_set_topo", "b200pf_series_step", "b200pf_series_results",
-               "b200pf_series_fetch", "b200pf_sync", "b200pf_last_launch_info", "b200pf_staging", "b200pf_run_staged",
+               "b200pf_series_fetch", "b200pf_sync", "b200pf_last_launch_info", "b200pf_last_launch_config", "b200pf_staging", "b200pf_run_staged",
                "b200pf_series_bind_outputs", "b200pf_set_stream", "b200pf_set_static_inj", "b200pf_rows_staging",
                "b200pf_run_rows_staged", "b200pf_set_thermal_limit", "b200pf_n1_host", "b200pf_series_protections",
                "b200pf_series_next_is_reset", "b200pf_series_fetch_state", "b200pf_rows_chunk_launch", "b200pf_rows_chunk_wait",
@@ -622,9 +624,15 @@ class PowerFlowEngine:
         return int(self.lib.b200pf_launch_count(self.h))
 
     def last_launch_info(self):
+        """Launch configuration of the last planned / pivoting launch.  ``config``: its kernel's template parameters
+        (``b200pf_last_launch_config``) — block kernel (T, U, MINB, PROT, WPC, STAGE, UNI, MODE), scalar planned kernel
+        (T, -1, MINB, PROT, -1, ...), pivoting kernels all -1."""
         v = [C.c_int() for _ in range(4)]
         self.lib.b200pf_last_launch_info(self.h, *[C.byref(x) for x in v])
-        return dict(smem_bytes=v[0].value, threads_per_instance=v[1].value, grid=v[2].value, block=v[3].value)
+        cfg = (C.c_int * 8)()
+        self._check(self.lib.b200pf_last_launch_config(self.h, cfg), "b200pf_last_launch_config")
+        return dict(smem_bytes=v[0].value, threads_per_instance=v[1].value, grid=v[2].value, block=v[3].value,
+                    config=tuple(int(x) for x in cfg))
 
     KERNEL_AUTO, KERNEL_PIVOTING, KERNEL_PLANNED = 0, 1, 2
 

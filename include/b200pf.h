@@ -338,6 +338,13 @@ int64_t b200pf_launch_count(const b200pf_handle *h);
 /* dynamic shared memory bytes and threads-per-instance the last launch used (diagnostics) */
 int b200pf_last_launch_info(const b200pf_handle *h, int *smem_bytes, int *threads_per_instance,
                             int *grid_blocks, int *block_threads);
+/* template parameters of the kernel the last launch ran (diagnostics; tests read which dispatch branch was taken), 8 ints:
+ * block kernel (pf_kernel_block): T (lanes per instance), U (operations per lane and row), MINB (resident CTAs the register
+ * budget is compiled for), PROT, WPC (warps per CTA), STAGE (shared plan copied into shared memory), UNI (lockstep warps),
+ * MODE (1: AC solve fed by chronics rows); scalar planned kernel (pf_kernel_sparse): T, -1, MINB, PROT, -1, -1, -1, -1;
+ * pivoting kernels: all -1.  With b200pf_last_launch_info, the launch ran ceil(batch / (grid_blocks * block_threads /
+ * threads_per_instance)) waves: rounds of its persistent CTAs. */
+int b200pf_last_launch_config(const b200pf_handle *h, int *cfg8);
 
 #ifdef __cplusplus
 }
