@@ -108,6 +108,10 @@ class BatchedEnv(BatchedDoNothing):
         self.current_step = np.zeros(B, dtype=np.int32)                    # env.nb_time_step (obs.current_step)
         self.soft_overflow_threshold = float(kw.get("soft_overflow_threshold", 1.0))
         self._obs = None
+        # tensor path (:meth:`step_tensors`): device buffers of the per-instance state, and where that state lives now ("host" or
+        # "device"); a host-path call pulls it, the next step_tensors pushes it back
+        self._dev = None
+        self._authority = "host"
 
     # ------------------------------------------------------------------------------------------------------------
     def _bus_cap(self) -> int:
@@ -127,10 +131,12 @@ class BatchedEnv(BatchedDoNothing):
         return min(n, self.gm.n_slot)
 
     def line_status(self) -> np.ndarray:
+        self._to_host()
         return (self.topo[:, self.line_or_pos] > 0) & (self.topo[:, self.line_ex_pos] > 0)
 
     def _apply_agent(self, sub_id, sub_bus, line_id, line_status):
         """-> (aff_lines bool [B, n_line], aff_subs bool [B, n_sub]) of the LEGAL actions, applied to self.topo"""
+        self._to_host()
         gm, B = self.gm, self.batch
         aff_l = np.zeros((B, gm.n_line), dtype=bool)
         aff_s = np.zeros((B, gm.n_sub), dtype=bool)
@@ -265,6 +271,7 @@ class BatchedEnv(BatchedDoNothing):
         element of that substation in topology-vector order, 0 = leave); ``line_id`` int [B] (-1: none) with ``line_status``
         int [B] (+1 reconnect / -1 disconnect).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the
         device (:meth:`fetch`)."""
+        self._to_host()
         gm = self.gm
         aff_l, aff_s = self._apply_agent(sub_id, sub_bus, line_id, line_status) if not from_reset else (
             np.zeros((self.batch, gm.n_line), dtype=bool), np.zeros((self.batch, gm.n_sub), dtype=bool))
@@ -334,6 +341,7 @@ class BatchedEnv(BatchedDoNothing):
         attached to (it zeroes the voltage of open lines, not the angle: pandaPowerBackend.py:1163-1187), 0 when that busbar has no
         element left.  Same rule as ``B200Backend._theta_of_open_lines``, for the whole batch."""
         from .engine import OutputView
+        self._to_host()
         gm, B = self.gm, self.batch
         v = OutputView(gm, out)
         th_or, th_ex = np.array(v.theta_or, dtype=np.float32), np.array(v.theta_ex, dtype=np.float32)
@@ -361,7 +369,12 @@ class BatchedEnv(BatchedDoNothing):
     def reset_instances(self, idx, rows=None):
         """``env.reset()`` of the instances ``idx`` (typically the finished ones): plain topology, cooldowns / counters / done flag
         cleared on the host and on the device, next chronics row ``rows`` (default: the row each instance started from).  Their
-        next :meth:`step` is an ordinary step on that row (use ``rows - 1`` semantics of your agent loop accordingly)."""
+        next :meth:`step` is an ordinary step on that row (use ``rows - 1`` semantics of your agent loop accordingly).
+        ``idx`` may also be a CUDA bool mask [B] (``rows``: None or a CUDA integer tensor [B]): the reset then runs on the device
+        (:meth:`step_tensors`)."""
+        if _is_cuda_tensor(idx):
+            return self._reset_tensors(idx, rows)
+        self._to_host()
         idx = np.asarray(idx, dtype=np.int64)
         if len(idx) == 0:
             return
@@ -416,6 +429,7 @@ class BatchedEnv(BatchedDoNothing):
     def observe_inputs(self) -> np.ndarray:
         """int32 [B, n_line + n_sub + 3]: the per-instance values only the host knows (cooldowns, current_step, step stamp, flags
         illegal / game over / reset) — what one observe launch copies to the device."""
+        self._to_host()
         gm, o = self.gm, self._obs
         h = o["host_in"]
         nl, ns = gm.n_line, gm.n_sub
@@ -432,6 +446,8 @@ class BatchedEnv(BatchedDoNothing):
         if self._obs is None:
             raise RuntimeError("call enable_observation() first")
         B, n_obs = self.batch, self._obs["n_obs"]
+        if self._authority == "device":
+            return self._observe_device(obs_out, reward_out)
         host_in = self.observe_inputs()
         if not hasattr(self.engine, "h"):                 # host-side engine (test infrastructure): numpy in / out
             obs, rew = self.engine.observe_host(host_in, obs_out, reward_out)
@@ -453,9 +469,203 @@ class BatchedEnv(BatchedDoNothing):
         self._obs["reset"][:] = False
         return obs, rew
 
+    def _observe_device(self, obs_out, reward_out):
+        """:meth:`observe` in tensor mode: the input record the last step wrote on the device, no host copy"""
+        import torch
+        B, n_obs = self.batch, self._obs["n_obs"]
+        dev = self._dev["device"]
+        obs = obs_out if obs_out is not None else torch.empty((B, n_obs), dtype=torch.float32, device=dev)
+        rew = reward_out if reward_out is not None else torch.empty(B, dtype=torch.float32, device=dev)
+        _check_tensor(obs, "obs_out", (B, n_obs), (torch.float32,), dev)
+        _check_tensor(rew, "reward_out", (B,), (torch.float32,), dev)
+        if not (obs.is_contiguous() and rew.is_contiguous()):
+            raise ValueError("obs_out / reward_out must be contiguous")
+        cur, eng = self._streams()
+        eng.wait_stream(cur)
+        self.engine.observe_device(obs.data_ptr(), rew.data_ptr())
+        cur.wait_stream(eng)
+        return obs, rew
+
+    # ---- tensor path: actions in, state out, as CUDA tensors ------------------------------------------------------------
+    def _streams(self):
+        import torch
+        dev = self._dev["device"]
+        return torch.cuda.current_stream(dev), torch.cuda.ExternalStream(self.engine.stream, device=dev)
+
+    def _tensor_state(self):
+        """the device buffers of the per-instance state, bound to the engine on first use"""
+        if self._dev is not None:
+            return self._dev
+        if not hasattr(self.engine, "h"):
+            raise RuntimeError("step_tensors needs the CUDA engine")
+        import torch
+        gm, B = self.gm, self.batch
+        dev = torch.device("cuda", getattr(self.engine, "device", 0))
+        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)       # noqa: E731
+        st = dict(last_bus=z((B, gm.dim_topo), torch.int8), line_cd=z((B, gm.n_line), torch.int32), sub_cd=z((B, gm.n_sub), torch.int32),
+                  done=z(B, torch.bool), is_illegal=z(B, torch.bool), newly_done=z(B, torch.bool), current_step=z(B, torch.int32),
+                  status=z(B, torch.int32))
+        if self._iso_cols is None:
+            self._isolated_shunt_busbar()                 # (builds the column segments)
+        tables = dict(sub_pos=self.sub_pos, line_of_pos=self.line_of_pos, other_end_pos=self.other_end_pos, cd_line=self.cd_line,
+                      cd_sub=self.cd_sub, cd_reco=self.cd_reco, maint=self._maint, haz=self._haz, maint_time=self._maint_time,
+                      maint_dur=self._maint_dur, haz_dur=self._haz_dur, iso_seg=self._iso_seg, iso_cols=self._iso_cols,
+                      topo0=self.topo0, t0=self.t0)
+        self.engine.env_bind(tables, {k: v.data_ptr() for k, v in st.items()})
+        p, q = self.engine.series_device_pointers(), self.engine.env_pointers()
+        st["rho"] = _device_view(p["rho"], (B, gm.n_line), "<f4", dev)
+        st["iters"] = _device_view(p["iters"], (B,), "<i4", dev)
+        st["disc"] = _device_view(q["disc"], (B, gm.n_line), "<i4", dev)
+        st["device"] = dev
+        self._dev = st
+        self._illegal_seen = 0
+        return st
+
+    def _to_device(self):
+        """hand the host state to the tensor path"""
+        import torch
+        d = self._tensor_state()
+        if self._authority == "device":
+            return
+        for name, arr in (("last_bus", self.last_bus), ("line_cd", self.line_cooldown), ("sub_cd", self.sub_cooldown), ("done", self.done),
+                          ("is_illegal", self.is_illegal), ("current_step", self.current_step)):
+            d[name].copy_(torch.from_numpy(np.ascontiguousarray(arr)))
+        torch.cuda.current_stream(d["device"]).synchronize()
+        obs = self._obs is not None
+        self.engine.env_set_state(self.topo, self._nb_inst, self._cap_dirty, self._obs["reset"] if obs else None,
+                                  self.observe_inputs() if obs else None)
+        self._illegal_seen = self.engine.env_stats()["n_illegal"]
+        self._authority = "device"
+
+    def _to_host(self):
+        """hand the tensor path's state to the host path"""
+        if self._authority != "device":
+            return
+        d = self._dev
+        s = self.engine.env_get_state()                   # (waits for the engine's stream)
+        self._authority = "host"
+        self.topo[:] = s["topo"]
+        self.row = s["t"].astype(np.int64)
+        self.last_bus[:] = d["last_bus"].cpu().numpy(); self.line_cooldown[:] = d["line_cd"].cpu().numpy()
+        self.sub_cooldown[:] = d["sub_cd"].cpu().numpy(); self.done[:] = d["done"].cpu().numpy()
+        self.is_illegal = d["is_illegal"].cpu().numpy().copy(); self.current_step[:] = d["current_step"].cpu().numpy()
+        self._nb_inst[:] = s["nb_inst"]; self._cap_dirty[:] = s["cap_dirty"]
+        if self._obs is not None:
+            self._obs["reset"][:] = s["obs_reset"]
+        if self.tight_cap and self._cap_dirty.any():
+            self.nb_cap = self._bus_cap()
+
+    def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False):
+        """:meth:`step` with the actions as CUDA tensors and the state kept on the device: ``sub_id`` int32 / int64 [B] (-1: none)
+        with ``sub_bus`` int8 / int32 / int64 [B, >= max_sub_size]; ``line_id`` int32 / int64 [B] (-1: none) with ``line_status``
+        int32 / int64 [B] (> 0 reconnect / < 0 disconnect).  Same semantics and bit-identical state as :meth:`step`; ordered against torch's current
+        stream.  Returns ``(rho [B, n_line], done [B], info)`` as CUDA tensors; ``info``: ``status`` (with the isolated-busbar
+        override), ``iters``, ``newly_done``, ``is_illegal``, ``disc_lines`` (protections on, else None).  The returned tensors
+        are the environment's own buffers: the next step overwrites them.  The host waits once per step for a few words (and
+        copies back the changed topology rows when the plans have to be looked up, which waits again).  An id or busbar out of
+        range raises ValueError and changes nothing."""
+        import torch
+        d = self._tensor_state()
+        dev, B = d["device"], self.batch
+        if (sub_id is None) != (sub_bus is None) or (line_id is None) != (line_status is None):
+            raise ValueError("sub_id / sub_bus and line_id / line_status come in pairs")
+        ints = (torch.int32, torch.int64)
+        keep = []
+
+        def ids(x, name):
+            _check_tensor(x, name, (B,), ints, dev)
+            y = x if x.dtype == torch.int32 else x.clamp(-2 ** 31, 2 ** 31 - 1).to(torch.int32)   # (out of range stays out of range)
+            y = y.contiguous()
+            keep.append(y)
+            return y.data_ptr()
+
+        sid = sbus = lid = lst = 0
+        cols = stride = 0
+        if sub_id is not None:
+            sid = ids(sub_id, "sub_id")
+            if not (torch.is_tensor(sub_bus) and sub_bus.is_cuda and sub_bus.device == dev and sub_bus.dim() == 2 and sub_bus.shape[0] == B
+                    and sub_bus.shape[1] >= self.max_sub_size and sub_bus.dtype in (torch.int8,) + ints):
+                raise ValueError(f"sub_bus must be an int8 / int32 / int64 CUDA tensor of shape ({B}, >= {self.max_sub_size}) on {dev}")
+            sb = sub_bus if sub_bus.dtype == torch.int8 else sub_bus.clamp(-128, 127).to(torch.int8)
+            if sb.stride(1) != 1:
+                sb = sb.contiguous()
+            keep.append(sb)
+            sbus, cols, stride = sb.data_ptr(), sb.shape[1], sb.stride(0)
+        if line_id is not None:
+            lid = ids(line_id, "line_id")
+            lst = ids(line_status, "line_status")
+        if self._authority != "device":
+            self._to_device()
+        cur, eng = self._streams()
+        eng.wait_stream(cur)
+        try:
+            self.engine.env_step(sid, sbus, stride, cols, lid, lst, from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter,
+                                 tol_mva=self.tol_mva, tight_cap=self.tight_cap, stamp=self.n_steps + 1)
+        except RuntimeError as e:
+            if "(-1)" in str(e):                          # B200PF_E_ARG: an action out of range, nothing was written
+                raise ValueError(str(e)) from None
+            raise
+        cur.wait_stream(eng)
+        self.n_steps += 1
+        self._n_dev_steps = getattr(self, "_n_dev_steps", 0) + 1     # (as step_device counts them: simulate_forecast reads it)
+        st = self.engine.env_stats()
+        self.n_illegal += st["n_illegal"] - self._illegal_seen
+        self._illegal_seen = st["n_illegal"]
+        if self.tight_cap:
+            self.nb_cap = st["nb_cap"]
+        info = {"status": d["status"], "iters": d["iters"], "newly_done": d["newly_done"], "is_illegal": d["is_illegal"],
+                "disc_lines": d["disc"] if self.protections else None}
+        return d["rho"], d["done"], info
+
+    def _reset_tensors(self, mask, rows=None):
+        import torch
+        d = self._tensor_state()
+        dev, B = d["device"], self.batch
+        _check_tensor(mask, "mask", (B,), (torch.bool,), dev)
+        m = mask.contiguous()
+        r = None
+        if rows is not None:
+            _check_tensor(rows, "rows", (B,), (torch.int32, torch.int64), dev)
+            r = torch.remainder(rows, self.chron.shape[1]).to(torch.int32).contiguous()
+        if self._authority != "device":
+            self._to_device()
+        cur, eng = self._streams()
+        eng.wait_stream(cur)
+        self.engine.env_reset(m.data_ptr(), 0 if r is None else r.data_ptr())
+        cur.wait_stream(eng)
+        m.record_stream(eng)                              # (the mask / rows may be freed before the engine's stream read them)
+        if r is not None:
+            r.record_stream(eng)
+
     def reset_step(self):
         """the solve ``env.reset()`` performs on the first row (no soft-overflow counting, no cooldown from actions)"""
         return self.step(from_reset=True)
+
+
+def _is_cuda_tensor(x) -> bool:
+    try:
+        import torch
+    except ImportError:                                   # pragma: no cover
+        return False
+    return torch.is_tensor(x) and x.is_cuda
+
+
+def _check_tensor(x, name, shape, dtypes, device):
+    import torch
+    if not (torch.is_tensor(x) and x.is_cuda and x.device == device and tuple(x.shape) == tuple(shape) and x.dtype in dtypes):
+        raise ValueError(f"{name} must be a CUDA tensor of shape {tuple(shape)} and dtype {' / '.join(str(t) for t in dtypes)} on {device}")
+
+
+class _DeviceArray:
+    """``__cuda_array_interface__`` of device memory the engine owns (zero-copy torch views)"""
+
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = dict(shape=tuple(shape), typestr=typestr, data=(int(ptr), False), version=2, strides=None)
+
+
+def _device_view(ptr, shape, typestr, device):
+    import torch
+    return torch.as_tensor(_DeviceArray(ptr, shape, typestr), device=device)
 
 
 def random_substation_actions(env: BatchedEnv, rng: np.random.Generator):

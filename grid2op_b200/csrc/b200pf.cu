@@ -7,6 +7,7 @@
 #include "b200pf_block.cuh"
 #include "b200pf_redo.cuh"
 #include "b200pf_obs.cuh"
+#include "b200pf_env.cuh"
 #include "../../include/b200pf.h"
 
 #include <cstdio>
@@ -111,6 +112,15 @@ struct b200pf_handle {
     int32_t *h_obs_in = nullptr, *d_obs_in = nullptr;       // pinned host record of the per-instance inputs and its device copy
     cudaEvent_t obs_ev = nullptr; bool obs_ev_pending = false;
     int64_t obs_launches = 0, obs_h2d_bytes = 0, d2h_bytes = 0;
+    // device environment state (b200pf_env_bind / b200pf_env_step)
+    EnvArgs env{}; int env_batch = 0;
+    std::vector<void *> env_allocs;
+    int32_t *h_env_ctl = nullptr;                           // pinned copy of the step's control words
+    std::vector<int8_t> env_mirror;                         // host mirror of the device topology the plans are looked up from
+    std::vector<int32_t> env_list; std::vector<int8_t> env_rows;
+    std::vector<int8_t> env_topo0; std::vector<uint8_t> env_mask;   // host copies: reset topologies, the last reset mask
+    int64_t env_steps = 0, env_h2d = 0, env_d2h = 0, env_waits = 0, env_illegal = 0, env_plan_refresh = 0;
+    int env_last_cap = 0, env_last_dirty = 0;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -319,6 +329,8 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     for (void *p : h->obs_allocs) cudaFree(p);
     if (h->h_obs_in) cudaFreeHost(h->h_obs_in);
     if (h->obs_ev) cudaEventDestroy(h->obs_ev);
+    for (void *p : h->env_allocs) cudaFree(p);
+    if (h->h_env_ctl) cudaFreeHost(h->h_env_ctl);
     delete h;
     return 0;
 }
@@ -1828,5 +1840,292 @@ extern "C" int b200pf_last_launch_info(const b200pf_handle *h, int *smem_bytes, 
 extern "C" int b200pf_last_launch_config(const b200pf_handle *h, int *cfg8) {
     if (!h || !cfg8) return fail(B200PF_E_ARG, "null pointer");
     for (int k = 0; k < 8; ++k) cfg8[k] = h->last_cfg[k];
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// device environment state: BatchedEnv's bookkeeping on the device (b200pf_env.cuh)
+// ------------------------------------------------------------------------------------------------
+static bool env_bound(const b200pf_handle *h) { return h->env_batch && h->env_batch == h->series_batch && h->env.topo == h->d_series_topo; }
+
+extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
+    const DevGrid &g = h->g;
+    if (d->max_sub <= 0 || !d->sub_pos || !d->line_of_pos || !d->other_end_pos || !d->topo0 || !d->t0 || (d->n_iso_seg && !d->iso_seg) ||
+        (d->n_iso_cols && !d->iso_cols) || d->n_iso_seg < 0 || d->n_iso_cols < 0 || (!d->maint) != (!d->maint_time) || (d->maint && !d->maint_dur) ||
+        (!d->haz) != (!d->haz_dur))
+        return fail(B200PF_E_ARG, "bad environment tables");
+    if (!d->last_bus || !d->line_cd || !d->sub_cd || !d->done || !d->is_illegal || !d->newly_done || !d->current_step || !d->status)
+        return fail(B200PF_E_ARG, "state buffers missing");
+    if (g.n_slot > ENV_MAX_SLOT) return fail(B200PF_E_CAPACITY, "more bus slots than the device bus count handles");
+    for (int k = 0; k < g.n_sub * d->max_sub; ++k) if (d->sub_pos[k] < -1 || d->sub_pos[k] >= g.dim_topo) return fail(B200PF_E_ARG, "sub_pos out of range");
+    for (int k = 0; k < g.dim_topo; ++k)
+        if (d->line_of_pos[k] < -1 || d->line_of_pos[k] >= g.n_line || d->other_end_pos[k] < -1 || d->other_end_pos[k] >= g.dim_topo)
+            return fail(B200PF_E_ARG, "line_of_pos / other_end_pos out of range");
+    for (int k = 0; k < d->n_iso_cols; ++k) if (d->iso_cols[k] < 0 || d->iso_cols[k] >= g.n_topo_in) return fail(B200PF_E_ARG, "iso_cols out of range");
+    for (int k = 0; k < d->n_iso_seg; ++k) if (d->iso_seg[k] < 0 || d->iso_seg[k] > d->n_iso_cols) return fail(B200PF_E_ARG, "iso_seg out of range");
+    const int B = h->series_batch;
+    for (int i = 0; i < B; ++i) if (d->t0[i] < 0 || d->t0[i] >= h->n_rows) return fail(B200PF_E_ARG, "t0 out of range");
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (void *p : h->env_allocs) cudaFree(p);
+    h->env_allocs.clear();
+    h->env_batch = 0;
+    if (!h->h_env_ctl && cudaMallocHost(&h->h_env_ctl, ENV_CTL_WORDS * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
+    auto dup = [&](const void *src, size_t bytes, void **dst) -> int {
+        *dst = nullptr;
+        if (!src) return 0;
+        CU(cudaMalloc(dst, bytes ? bytes : 1));
+        h->env_allocs.push_back(*dst);
+        if (bytes) H2D(*dst, src, bytes);
+        return 0;
+    };
+    auto zeros = [&](size_t bytes, int byte, void **dst) -> int {
+        CU(cudaMalloc(dst, bytes ? bytes : 1));
+        h->env_allocs.push_back(*dst);
+        CU(cudaMemsetAsync(*dst, byte, bytes ? bytes : 1, h->stream));
+        return 0;
+    };
+    std::vector<int32_t> epos, esub;           // every element of the record and its substation (b200pf_grid_max_active_buses)
+    const HostGrid &hg = h->hg;
+    for (int k = 0; k < hg.n_line; ++k) { epos.push_back(hg.line_or_pos[k]); esub.push_back(hg.line_or_sub[k]); }
+    for (int k = 0; k < hg.n_line; ++k) { epos.push_back(hg.line_ex_pos[k]); esub.push_back(hg.line_ex_sub[k]); }
+    for (int k = 0; k < hg.n_unit; ++k) { epos.push_back(hg.unit_pos[k]); esub.push_back(hg.unit_sub[k]); }
+    for (int k = 0; k < hg.n_load; ++k) { epos.push_back(hg.load_pos[k]); esub.push_back(hg.load_sub[k]); }
+    for (int k = 0; k < hg.n_sto; ++k) { epos.push_back(hg.sto_pos[k]); esub.push_back(hg.sto_sub[k]); }
+    for (int k = 0; k < hg.n_shunt; ++k) { epos.push_back(hg.dim_topo + k); esub.push_back(hg.sh_sub[k]); }
+    const size_t R = (size_t)h->n_scen * h->n_rows * g.n_line, nl = (size_t)g.n_line, nt = (size_t)g.n_topo_in;
+    EnvArgs a{};
+    void *p[32] = {};
+    int rc;
+    if ((rc = dup(d->sub_pos, (size_t)g.n_sub * d->max_sub * 4, &p[0])) || (rc = dup(d->line_of_pos, (size_t)g.dim_topo * 4, &p[1])) ||
+        (rc = dup(d->other_end_pos, (size_t)g.dim_topo * 4, &p[2])) || (rc = dup(epos.data(), epos.size() * 4, &p[3])) ||
+        (rc = dup(esub.data(), esub.size() * 4, &p[4])) || (rc = dup(d->maint, R, &p[5])) || (rc = dup(d->haz, R, &p[6])) ||
+        (rc = dup(d->maint_time, R * 4, &p[7])) || (rc = dup(d->maint_dur, R * 4, &p[8])) || (rc = dup(d->haz_dur, R * 4, &p[9])) ||
+        (rc = dup(d->iso_cols, (size_t)d->n_iso_cols * 4, &p[10])) || (rc = dup(d->iso_seg, (size_t)d->n_iso_seg * 4, &p[11])) ||
+        (rc = dup(d->topo0, (size_t)B * nt, &p[12])) || (rc = dup(d->t0, (size_t)B * 4, &p[13])) ||
+        (rc = zeros((size_t)B * nl, 0, &p[14])) || (rc = zeros((size_t)B * 4, 0xff, &p[15])) || (rc = zeros((size_t)B * 4, 0, &p[16])) ||
+        (rc = zeros((size_t)B, 0, &p[17])) || (rc = zeros((size_t)B, 1, &p[18])) || (rc = zeros((size_t)B, 1, &p[19])) ||
+        (rc = zeros((size_t)B * 4, 0, &p[20])) || (rc = zeros((size_t)B * 4, 0, &p[21])) || (rc = zeros((size_t)B * nt, 0, &p[22])) ||
+        (rc = zeros(ENV_CTL_WORDS * 4, 0, &p[23])))
+        return rc;
+    a.batch = B;
+    a.n_line = g.n_line; a.n_sub = g.n_sub; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_busbar = g.n_busbar; a.n_slot = g.n_slot;
+    a.max_sub = d->max_sub; a.n_rows = h->n_rows;
+    a.sub_pos = (const int32_t *)p[0]; a.line_of_pos = (const int32_t *)p[1]; a.other_end_pos = (const int32_t *)p[2];
+    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
+    a.elem_pos = (const int32_t *)p[3]; a.elem_sub = (const int32_t *)p[4]; a.n_elem = (int)epos.size();
+    a.cd_line = d->cd_line; a.cd_sub = d->cd_sub; a.cd_reco = d->cd_reco;
+    a.maint = (const uint8_t *)p[5]; a.haz = (const uint8_t *)p[6];
+    a.maint_time = (const int32_t *)p[7]; a.maint_dur = (const int32_t *)p[8]; a.haz_dur = (const int32_t *)p[9];
+    a.iso_cols = (const int32_t *)p[10]; a.iso_seg = (const int32_t *)p[11]; a.n_iso_seg = d->n_iso_seg; a.n_iso_cols = d->n_iso_cols;
+    a.topo0 = (const int8_t *)p[12]; a.t0 = (const int32_t *)p[13]; a.scen = h->d_scen;
+    a.topo = h->d_series_topo; a.t = h->d_t;
+    a.lib_done = h->d_done; a.pcount = h->d_pcount; a.ts_over = h->d_tsover; a.lib_disc = h->d_disc; a.trip = h->d_trip; a.incdone = h->d_incdone;
+    a.last_bus = d->last_bus; a.line_cd = d->line_cd; a.sub_cd = d->sub_cd; a.done = d->done; a.is_illegal = d->is_illegal;
+    a.newly_done = d->newly_done; a.current_step = d->current_step; a.status_out = d->status;
+    a.aff_l = (uint8_t *)p[14]; a.aff_s = (int32_t *)p[15]; a.row_used = (int32_t *)p[16];
+    a.stale = (uint8_t *)p[17]; a.cap_dirty = (uint8_t *)p[18]; a.obs_reset = (uint8_t *)p[19];
+    a.nb_inst = (int32_t *)p[20]; a.copy_list = (int32_t *)p[21]; a.copy_rows = (int8_t *)p[22]; a.ctl = (int32_t *)p[23];
+    // the stale flags start set: the first step that refreshes the plans copies every row into the mirror
+    CU(cudaMemsetAsync(a.stale, 1, (size_t)B, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->env = a; h->env_batch = B;
+    h->env_mirror.assign((size_t)B * nt, 0);
+    h->env_topo0.assign(d->topo0, d->topo0 + (size_t)B * nt);
+    return 0;
+}
+
+static inline unsigned env_grid(int n) { return (unsigned)((n + 127) / 128); }
+
+extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
+                               const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter,
+                               double tol_mva, int tight_cap, int stamp) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
+    if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
+    CU(cudaSetDevice(h->device));
+    const DevGrid &g = h->g;
+    const int B = h->env_batch;
+    const size_t nt = (size_t)g.n_topo_in;
+    EnvArgs a = h->env;
+    a.sub_id = from_reset ? nullptr : d_sub_id; a.sub_bus = from_reset ? nullptr : d_sub_bus;
+    a.sub_bus_stride = sub_bus_stride; a.sub_bus_cols = sub_bus_cols;
+    a.line_id = from_reset ? nullptr : d_line_id; a.line_status = from_reset ? nullptr : d_line_status;
+    a.from_reset = from_reset ? 1 : 0; a.tight_cap = tight_cap ? 1 : 0; a.prot = h->prot;
+    // 1. validation + apply (the apply kernel writes nothing when an input was rejected)
+    CU(cudaMemsetAsync(a.ctl, 0, ENV_CTL_WORDS * 4, h->stream));
+    if (a.sub_id || a.line_id) {
+        pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
+        CU(cudaGetLastError());
+    }
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a);
+    CU(cudaGetLastError());
+    // 2. the step's one host wait: dirty count, bus cap, input error
+    CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->env_d2h += ENV_CTL_WORDS * 4; h->env_waits++;
+    const int32_t *c = h->h_env_ctl;
+    if (c[ENV_CTL_ERR]) return fail(B200PF_E_ARG, "action out of range (substation / line id outside [-1, n), busbar outside [-1, n_busbar])");
+    h->env_illegal += c[ENV_CTL_N_ILLEGAL];
+    int nb_cap = 0;
+    if (tight_cap) {
+        nb_cap = c[ENV_CTL_CAP_MAX];
+        if (nb_cap > 17) nb_cap = (nb_cap + 7) / 8 * 8;
+        if (nb_cap > g.n_slot) nb_cap = g.n_slot;
+    }
+    h->env_last_cap = nb_cap; h->env_last_dirty = c[ENV_CTL_N_DIRTY];
+    // 3.-4. a changed topology: patch the mirror with the compacted rows, then the plans of the full mirror (as series_set_topo)
+    if (c[ENV_CTL_N_DIRTY] > 0) {
+        const int n = c[ENV_CTL_N_COPY];
+        if (n < 0 || n > B) return fail(B200PF_E_STATE, "bad row count");
+        if (n) {
+            h->env_list.resize(n); h->env_rows.resize((size_t)n * nt);
+            CU(cudaMemcpyAsync(h->env_list.data(), a.copy_list, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
+            CU(cudaMemcpyAsync(h->env_rows.data(), a.copy_rows, (size_t)n * nt, cudaMemcpyDeviceToHost, h->stream));
+            CU(cudaMemsetAsync(a.stale, 0, (size_t)B, h->stream));
+            CU(cudaStreamSynchronize(h->stream));
+            h->env_d2h += (int64_t)n * (4 + (int64_t)nt); h->env_waits++;
+            for (int k = 0; k < n; ++k) {
+                const int i = h->env_list[k];
+                if (i < 0 || i >= B) return fail(B200PF_E_STATE, "bad instance in the row list");
+                memcpy(h->env_mirror.data() + (size_t)i * nt, h->env_rows.data() + (size_t)k * nt, nt);
+            }
+        }
+        int rc = series_plans(h, h->env_mirror.data());
+        if (rc) return rc;
+        h->series_dev_topo_ahead = false;
+        h->env_plan_refresh++;
+    }
+    // 5. the series step (kernel selection, protections, cascades and safety net unchanged)
+    h->next_reset = from_reset ? 1 : 0;
+    int rc = b200pf_series_step(h, is_dc, max_iter, tol_mva, nb_cap);
+    if (rc) return rc;
+    // 6. trips, isolated busbars, cooldowns, game over, the observe layer's input record
+    a.status = h->x_status ? h->x_status : h->d_status;
+    a.disc = h->prot ? h->d_disc : nullptr;
+    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
+    a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3; a.stamp = stamp;
+    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a);
+    CU(cudaGetLastError());
+    h->env_steps++;
+    return 0;
+}
+
+extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const int32_t *d_rows) {
+    if (!h || !d_mask) return fail(B200PF_E_ARG, "null pointer");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    CU(cudaSetDevice(h->device));
+    const DevGrid &g = h->g;
+    const int B = h->env_batch;
+    const size_t nt = (size_t)g.n_topo_in;
+    EnvArgs a = h->env;
+    a.reset_mask = d_mask; a.reset_rows = d_rows;
+    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
+    a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3;
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a);
+    CU(cudaGetLastError());
+    // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
+    // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
+    // it chooses depend on the new topologies of each call)
+    h->env_mask.resize(B);
+    CU(cudaMemcpyAsync(h->env_mask.data(), d_mask, (size_t)B, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->env_d2h += B; h->env_waits++;
+    std::vector<int8_t> all;
+    bool any = false;
+    for (int i = 0; i < B; ++i) any |= h->env_mask[i] != 0;
+    if (!any) return 0;
+    if (h->series_dev_topo_ahead || h->h_series_topo.size() != (size_t)B * nt) {
+        all.resize((size_t)B * nt);
+        CU(cudaMemcpy(all.data(), h->d_series_topo, all.size(), cudaMemcpyDeviceToHost));
+        h->env_d2h += (int64_t)all.size();
+    } else all = h->h_series_topo;
+    for (int i = 0; i < B; ++i)
+        if (h->env_mask[i]) memcpy(all.data() + (size_t)i * nt, h->env_topo0.data() + (size_t)i * nt, nt);
+    h->series_dev_topo_ahead = false;
+    return series_plans(h, all.data());
+}
+
+extern "C" int b200pf_env_get_state(b200pf_handle *h, int8_t *topo, int32_t *t, int32_t *nb_inst, uint8_t *cap_dirty, uint8_t *obs_reset) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    CU(cudaSetDevice(h->device));
+    const size_t B = (size_t)h->env_batch, nt = (size_t)h->g.n_topo_in;
+    CU(cudaStreamSynchronize(h->stream));
+    if (topo) CU(cudaMemcpy(topo, h->d_series_topo, B * nt, cudaMemcpyDeviceToHost));
+    if (t) CU(cudaMemcpy(t, h->d_t, B * 4, cudaMemcpyDeviceToHost));
+    if (nb_inst) CU(cudaMemcpy(nb_inst, h->env.nb_inst, B * 4, cudaMemcpyDeviceToHost));
+    if (cap_dirty) CU(cudaMemcpy(cap_dirty, h->env.cap_dirty, B, cudaMemcpyDeviceToHost));
+    if (obs_reset) CU(cudaMemcpy(obs_reset, h->env.obs_reset, B, cudaMemcpyDeviceToHost));
+    h->env_d2h += (int64_t)((topo ? B * nt : 0) + (t ? B * 4 : 0) + (nb_inst ? B * 4 : 0) + (cap_dirty ? B : 0) + (obs_reset ? B : 0));
+    return 0;
+}
+
+extern "C" int b200pf_env_set_state(b200pf_handle *h, const int8_t *topo, const int32_t *nb_inst, const uint8_t *cap_dirty, const uint8_t *obs_reset,
+                                    const int32_t *obs_in) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    CU(cudaSetDevice(h->device));
+    const size_t B = (size_t)h->env_batch, nt = (size_t)h->g.n_topo_in;
+    if (topo) {
+        H2D(h->d_series_topo, topo, B * nt);
+        h->env_mirror.assign(topo, topo + B * nt);
+        CU(cudaMemsetAsync(h->env.stale, 0, B, h->stream));
+    }
+    if (nb_inst) H2D(h->env.nb_inst, nb_inst, B * 4);
+    if (cap_dirty) H2D(h->env.cap_dirty, cap_dirty, B);
+    if (obs_reset) H2D(h->env.obs_reset, obs_reset, B);
+    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
+    const size_t rec = B * (size_t)(h->g.n_line + h->g.n_sub + 3) * 4;
+    if (obs_in && obs) {
+        if (h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));        // (b200pf_observe's copy into the same record has left)
+        H2D(h->d_obs_in, obs_in, rec);
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    h->env_h2d += (int64_t)((topo ? B * nt : 0) + (nb_inst ? B * 4 : 0) + (cap_dirty ? B : 0) + (obs_reset ? B : 0) + (obs_in && obs ? rec : 0));
+    return 0;
+}
+
+extern "C" int b200pf_env_pointers(b200pf_handle *h, int8_t **d_topo, int32_t **d_t, int32_t **d_disc) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
+    if (d_topo) *d_topo = h->d_series_topo;
+    if (d_t) *d_t = h->d_t;
+    if (d_disc) *d_disc = h->d_disc;
+    return 0;
+}
+
+extern "C" int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_reward) {
+    if (!h || !d_obs) return fail(B200PF_E_ARG, "null pointer");
+    if (!h->obs_batch || h->obs_batch != h->series_batch || h->obs_rows != h->n_rows)
+        return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    CU(cudaSetDevice(h->device));
+    const DevGrid &g = h->g;
+    ObsArgs a = h->obs;
+    a.batch = h->obs_batch;
+    a.n_line = g.n_line; a.n_sub = g.n_sub; a.n_gen = g.n_gen; a.n_hidden = g.n_hidden; a.n_load = g.n_load; a.n_sto = g.n_sto;
+    a.n_shunt = g.n_shunt; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_out = g.n_out;
+    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
+    a.out = h->x_out ? h->x_out : h->d_out; a.rho = h->x_rho ? h->x_rho : h->d_rho; a.topo = h->d_series_topo;
+    a.t = h->d_t; a.scen = h->d_scen; a.chron = h->d_chron; a.n_rows = h->n_rows; a.th_lim = h->d_thlim;
+    a.host = h->d_obs_in; a.obs = d_obs; a.reward = d_reward;
+    pf_kernel_observe<<<(a.batch + 3) / 4, 128, 0, h->stream>>>(a);
+    CU(cudaGetLastError());
+    EnvArgs e = h->env;                  // the reset flags have been consumed
+    e.obs_in = h->d_obs_in; e.obs_stride = a.host_stride;
+    pf_kernel_env_observed<<<env_grid(e.batch), 128, 0, h->stream>>>(e);
+    CU(cudaGetLastError());
+    h->obs_launches++;
+    return 0;
+}
+
+extern "C" int b200pf_env_stats(const b200pf_handle *h, int64_t *out8) {
+    if (!h || !out8) return fail(B200PF_E_ARG, "null pointer");
+    out8[0] = h->env_steps; out8[1] = h->env_h2d; out8[2] = h->env_d2h; out8[3] = h->env_waits;
+    out8[4] = h->env_illegal; out8[5] = h->env_last_cap; out8[6] = h->env_last_dirty; out8[7] = h->env_plan_refresh;
     return 0;
 }

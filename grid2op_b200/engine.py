@@ -37,7 +37,8 @@ ABI_SYMBOLS = (
     "b200pf_set_debug", "b200pf_redo_launch_count",
     "b200pf_device_alloc", "b200pf_device_free", "b200pf_ipc_export", "b200pf_ipc_open", "b200pf_ipc_close", "b200pf_device_read", "b200pf_plan_counters", "b200pf_series_bind_flag",
     "b200pf_series_reset_instances", "b200pf_grid_max_active_buses", "b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats",
-    "b200pf_last_launch_config",
+    "b200pf_last_launch_config", "b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state",
+    "b200pf_env_set_state", "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats",
 )
 
 
@@ -74,6 +75,48 @@ class ObsDesc(C.Structure):
         ("max_regret", C.c_double), ("reward_min", C.c_double), ("reward_illegal", C.c_double), ("dts_hours", C.c_double),
         ("soft_thr", C.c_float),
     ]
+
+
+class EnvDesc(C.Structure):
+    """``b200pf_env_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("max_sub", C.c_int32), ("sub_pos", C.c_void_p), ("line_of_pos", C.c_void_p), ("other_end_pos", C.c_void_p),
+        ("cd_line", C.c_int32), ("cd_sub", C.c_int32), ("cd_reco", C.c_int32),
+        ("maint", C.c_void_p), ("haz", C.c_void_p), ("maint_time", C.c_void_p), ("maint_dur", C.c_void_p), ("haz_dur", C.c_void_p),
+        ("n_iso_seg", C.c_int32), ("n_iso_cols", C.c_int32), ("iso_seg", C.c_void_p), ("iso_cols", C.c_void_p),
+        ("topo0", C.c_void_p), ("t0", C.c_void_p),
+        ("last_bus", C.c_void_p), ("line_cd", C.c_void_p), ("sub_cd", C.c_void_p), ("done", C.c_void_p), ("is_illegal", C.c_void_p),
+        ("newly_done", C.c_void_p), ("current_step", C.c_void_p), ("status", C.c_void_p),
+    ]
+
+
+def make_env_desc(t: dict, state: dict):
+    """-> (``b200pf_env_desc`` for the static tables ``t`` (numpy, built by ``BatchedEnv``) and the per-instance device buffers
+    ``state`` (integer device addresses), the arrays it points to)"""
+    keep = []
+    d = EnvDesc()
+
+    def put(name, arr, dtype):
+        if arr is None:
+            setattr(d, name, None)
+            return
+        a = np.ascontiguousarray(arr, dtype=dtype)
+        if a.size == 0:
+            a = np.zeros(1, dtype=dtype)
+        keep.append(a)
+        setattr(d, name, a.ctypes.data)
+
+    d.max_sub = int(t["sub_pos"].shape[1])
+    put("sub_pos", t["sub_pos"], np.int32); put("line_of_pos", t["line_of_pos"], np.int32); put("other_end_pos", t["other_end_pos"], np.int32)
+    d.cd_line, d.cd_sub, d.cd_reco = int(t["cd_line"]), int(t["cd_sub"]), int(t["cd_reco"])
+    put("maint", t.get("maint"), np.uint8); put("haz", t.get("haz"), np.uint8)
+    put("maint_time", t.get("maint_time"), np.int32); put("maint_dur", t.get("maint_dur"), np.int32); put("haz_dur", t.get("haz_dur"), np.int32)
+    d.n_iso_seg, d.n_iso_cols = len(t["iso_seg"]), len(t["iso_cols"])
+    put("iso_seg", t["iso_seg"], np.int32); put("iso_cols", t["iso_cols"], np.int32)
+    put("topo0", t["topo0"], np.int8); put("t0", t["t0"], np.int32)
+    for name in ("last_bus", "line_cd", "sub_cd", "done", "is_illegal", "newly_done", "current_step", "status"):
+        setattr(d, name, int(state[name]))
+    return d, keep
 
 
 def make_obs_desc(t: dict):
@@ -195,6 +238,17 @@ def load_library():
     lib.b200pf_observe.argtypes = [vp, vp, vp, vp]
     lib.b200pf_obs_stats.argtypes = [vp, C.POINTER(C.c_int64)]
     for nm in ("b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats"):
+        getattr(lib, nm).restype = i32
+    lib.b200pf_env_bind.argtypes = [vp, C.POINTER(EnvDesc)]
+    lib.b200pf_env_step.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, i32, f64, i32, i32]
+    lib.b200pf_env_reset.argtypes = [vp, vp, vp]
+    lib.b200pf_env_get_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.b200pf_env_set_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.b200pf_env_pointers.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    lib.b200pf_observe_device.argtypes = [vp, vp, vp]
+    lib.b200pf_env_stats.argtypes = [vp, C.POINTER(C.c_int64)]
+    for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
+               "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -611,6 +665,57 @@ class PowerFlowEngine:
         v = (C.c_int64 * 4)()
         self._check(self.lib.b200pf_obs_stats(self.h, v), "b200pf_obs_stats")
         return dict(launches=int(v[0]), h2d_bytes=int(v[1]), d2h_bytes=int(v[2]), bytes_written_per_launch=int(v[3]))
+
+    # ---- device environment state ---------------------------------------------------------------
+    def env_bind(self, tables: dict, state: dict):
+        """Static tables + caller-owned per-instance device buffers of the device environment (``b200pf_env_bind``; built by
+        BatchedEnv)."""
+        d, keep = make_env_desc(tables, state)
+        self._check(self.lib.b200pf_env_bind(self.h, C.byref(d)), "b200pf_env_bind")
+        del keep
+
+    def env_step(self, sub_id: int = 0, sub_bus: int = 0, sub_bus_stride: int = 0, sub_bus_cols: int = 0, line_id: int = 0,
+                 line_status: int = 0, from_reset: bool = False, is_dc: bool = False, max_iter: int = 10, tol_mva: float = 1e-8,
+                 tight_cap: bool = True, stamp: int = 0):
+        """One env step of the bound series from device action buffers (integer addresses, 0 = none); one host wait."""
+        v = lambda x: C.c_void_p(int(x) or None)      # noqa: E731
+        self._check(self.lib.b200pf_env_step(self.h, v(sub_id), v(sub_bus), int(sub_bus_stride), int(sub_bus_cols), v(line_id),
+                                             v(line_status), int(bool(from_reset)), int(bool(is_dc)), int(max_iter), float(tol_mva),
+                                             int(bool(tight_cap)), int(stamp)), "b200pf_env_step")
+
+    def env_reset(self, d_mask: int, d_rows: int = 0):
+        self._check(self.lib.b200pf_env_reset(self.h, C.c_void_p(int(d_mask)), C.c_void_p(int(d_rows) or None)), "b200pf_env_reset")
+
+    def env_get_state(self):
+        """-> dict(topo int8 [B, n_topo_in], t int32 [B], nb_inst int32 [B], cap_dirty bool [B], obs_reset bool [B])"""
+        gm, B = self.gm, self._series_batch
+        topo = np.empty((B, gm.n_topo_in), np.int8); t = np.empty(B, np.int32); nb = np.empty(B, np.int32)
+        cd = np.empty(B, np.uint8); rs = np.empty(B, np.uint8)
+        self._check(self.lib.b200pf_env_get_state(self.h, _ptr(topo), _ptr(t), _ptr(nb), _ptr(cd), _ptr(rs)), "b200pf_env_get_state")
+        return dict(topo=topo, t=t, nb_inst=nb, cap_dirty=cd.astype(bool), obs_reset=rs.astype(bool))
+
+    def env_set_state(self, topo=None, nb_inst=None, cap_dirty=None, obs_reset=None, obs_in=None):
+        gm, B = self.gm, self._series_batch
+        a = None if topo is None else np.ascontiguousarray(topo, np.int8).reshape(B, gm.n_topo_in)
+        b = None if nb_inst is None else np.ascontiguousarray(nb_inst, np.int32)
+        c = None if cap_dirty is None else np.ascontiguousarray(cap_dirty, np.uint8)
+        r = None if obs_reset is None else np.ascontiguousarray(obs_reset, np.uint8)
+        o = None if obs_in is None else np.ascontiguousarray(obs_in, np.int32).reshape(B, gm.n_line + gm.n_sub + 3)
+        self._check(self.lib.b200pf_env_set_state(self.h, _ptr(a), _ptr(b), _ptr(c), _ptr(r), _ptr(o)), "b200pf_env_set_state")
+
+    def env_pointers(self):
+        p = [C.c_void_p() for _ in range(3)]
+        self._check(self.lib.b200pf_env_pointers(self.h, *[C.byref(x) for x in p]), "b200pf_env_pointers")
+        return dict(topo=p[0].value, t=p[1].value, disc=p[2].value)
+
+    def observe_device(self, d_obs: int, d_reward: int = 0):
+        self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")
+
+    def env_stats(self):
+        v = (C.c_int64 * 8)()
+        self._check(self.lib.b200pf_env_stats(self.h, v), "b200pf_env_stats")
+        return dict(steps=int(v[0]), h2d_bytes=int(v[1]), d2h_bytes=int(v[2]), host_waits=int(v[3]), n_illegal=int(v[4]),
+                    nb_cap=int(v[5]), n_dirty=int(v[6]), plan_refreshes=int(v[7]))
 
     def sync(self):
         self._check(self.lib.b200pf_sync(self.h), "b200pf_sync")

@@ -330,6 +330,65 @@ int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float
  * fetch / fetch_state), bytes one observe launch writes } */
 int b200pf_obs_stats(const b200pf_handle *h, int64_t *out4);
 
+/* Device environment state: BatchedEnv's bookkeeping for the bound series on the device (csrc/b200pf_env.cuh), so that an agent
+ * steps with device tensors and the host touches no per-instance data.  b200pf_env_bind copies the static tables below (host
+ * pointers) and keeps the per-instance state pointers: caller-owned DEVICE buffers (torch tensors, like
+ * b200pf_series_bind_outputs), which the kernels read and write in place.  Booleans are one byte (0 / 1).  A re-bound series
+ * needs a new b200pf_env_bind.
+ * b200pf_env_step, on the handle's stream: (1) one launch restating BatchedEnv._apply_agent + _apply_environment for every
+ * instance (DefaultRules legality, busbar writes, reconnections, line switching, maintenance / hazards of the row the solve uses,
+ * active-bus recount of the changed instances for the bus cap when tight_cap); (2) ONE host wait for a few control words;
+ * (3) when some topology changed (or a device reset happened since the last plan refresh): the changed rows, and the rows a trip or
+ * a reset changed since, are copied back to patch the host mirror of the device topology, and (4) the plans of the whole mirror are
+ * looked up exactly as b200pf_series_set_topo does; (5) the series step; (6) one launch for the rest of BatchedEnv.step: trips,
+ * the isolated-busbar status override, cooldowns, done / newly_done, current_step and the observe layer's input record (stamp =
+ * the caller's step number).  Actions: sub_id int32 [batch] (-1: none) with sub_bus int8 [batch][>= max_sub] (row stride
+ * sub_bus_stride bytes, sub_bus_cols columns), line_id int32 [batch] (-1: none) with line_status int32 [batch] (+1 / -1); either
+ * pair may be NULL.  A substation / line id outside [-1, n) or a busbar outside [-1, n_busbar] fails the call with B200PF_E_ARG
+ * before anything is written; any line status is accepted (> 0 reconnects, < 0 disconnects, 0 leaves the line, as the host path).
+ * b200pf_env_reset: env.reset() of the instances whose mask byte is 1 (topology and last busbars from topo0, cooldowns, done,
+ * current_step, is_illegal and the library's protection state cleared, next row rows[i] mod n_rows or t0[i] when rows is NULL),
+ * on the device.  The observe input record of those instances becomes what BatchedEnv.observe_inputs gives right after a reset.  The
+ * call then waits for the mask (batch bytes) and looks the plans of the reset rows up in the same call, over the same topology, as
+ * b200pf_series_reset_instances does for the host path, so that both paths build the same plans in the same calls.
+ * b200pf_env_get_state / b200pf_env_set_state: hand the state over to the host path and back (device topology, chronics row,
+ * active buses per instance, the instances waiting for a bus recount, the observe layer's reset flags; any pointer may be NULL;
+ * set_state's obs_in: the observe input record, int32 [batch][n_line + n_sub + 3], used when the observation layer is bound).
+ * b200pf_env_pointers: device topology, row index and disc_lines of
+ * the series (for zero-copy views).  b200pf_observe_device: b200pf_observe on the input record the last b200pf_env_step (or
+ * b200pf_env_reset) wrote, without a host copy; the reset flags it reported are cleared afterwards.
+ * b200pf_env_stats out8 = { env steps, bytes the env calls copied host-to-device, device-to-host, host waits of the env steps,
+ * illegal actions counted, bus cap of the last step, topology-changed instances of the last step, plan refreshes }. */
+typedef struct b200pf_env_desc {
+    int32_t max_sub;                    /* elements of the largest substation */
+    const int32_t *sub_pos;             /* [n_sub][max_sub] topology positions of each substation's elements, -1 padded */
+    const int32_t *line_of_pos, *other_end_pos;  /* [dim_topo] line whose end sits there (-1: none), position of its other end */
+    int32_t cd_line, cd_sub, cd_reco;   /* NB_TIMESTEP_COOLDOWN_LINE, NB_TIMESTEP_COOLDOWN_SUB, NB_TIMESTEP_RECONNECTION */
+    const uint8_t *maint, *haz;         /* [n_scen][n_rows][n_line] forced outages, or NULL */
+    const int32_t *maint_time, *maint_dur;  /* [n_scen][n_rows][n_line] (with maint) */
+    const int32_t *haz_dur;             /* [n_scen][n_rows][n_line] (with haz) */
+    int32_t n_iso_seg, n_iso_cols;      /* isolated-busbar rule: busbar 1 of these column segments must keep an element */
+    const int32_t *iso_seg, *iso_cols;  /* segment start offsets [n_iso_seg], topology columns [n_iso_cols] */
+    const int8_t *topo0;                /* [batch][n_topo_in] topology of a reset */
+    const int32_t *t0;                  /* [batch] row of a reset */
+    /* per-instance state: caller-owned device buffers */
+    int8_t *last_bus;                   /* [batch][dim_topo] */
+    int32_t *line_cd, *sub_cd;          /* [batch][n_line], [batch][n_sub] */
+    uint8_t *done, *is_illegal, *newly_done;  /* [batch] */
+    int32_t *current_step, *status;     /* [batch]; status: the step's status with the isolated-busbar override */
+} b200pf_env_desc;
+int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *desc);
+int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
+                    const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter, double tol_mva,
+                    int tight_cap, int stamp);
+int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const int32_t *d_rows);
+int b200pf_env_get_state(b200pf_handle *h, int8_t *topo, int32_t *t, int32_t *nb_inst, uint8_t *cap_dirty, uint8_t *obs_reset);
+int b200pf_env_set_state(b200pf_handle *h, const int8_t *topo, const int32_t *nb_inst, const uint8_t *cap_dirty, const uint8_t *obs_reset,
+                         const int32_t *obs_in);
+int b200pf_env_pointers(b200pf_handle *h, int8_t **d_topo, int32_t **d_t, int32_t **d_disc);
+int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_reward);
+int b200pf_env_stats(const b200pf_handle *h, int64_t *out8);
+
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */
 uint64_t b200pf_stream(b200pf_handle *h);

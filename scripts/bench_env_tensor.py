@@ -1,0 +1,138 @@
+"""Agent loop with actions: BatchedEnv.step fed by actions copied to the host, then observe, against BatchedEnv.step_tensors, then
+observe, alternating in one process.  Random one-substation and one-line actions drawn on the GPU with a seeded torch generator;
+protections off and on; case14 at batch 4096 and l2rpn_neurips_2020_track1 at batch 1024.  A host clock around K steps that end in
+a device synchronise, after warm-up.  Prints env.step/s (min / median / max over the repeats), the bytes each path copies per step,
+and the card and its power limit read in the same run.
+
+    python scripts/bench_env_tensor.py [--steps 50] [--warmup 5] [--repeats 5]
+"""
+import argparse
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+sys.path.insert(0, os.path.join(REPO, "tests"))
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=20)
+        return q.stdout.strip().splitlines()[0]
+    except Exception as e:                                    # pragma: no cover
+        return f"unknown ({e})"
+
+
+def draw(env, gen, dev):
+    import torch
+    B, gm = env.batch, env.gm
+    sub = torch.randint(0, gm.n_sub, (B,), generator=gen, device=dev, dtype=torch.int32)
+    bus = torch.randint(1, 3, (B, env.max_sub_size), generator=gen, device=dev, dtype=torch.int8)
+    size = torch.as_tensor(env.sub_size, device=dev)[sub.long()]
+    bus[torch.arange(env.max_sub_size, device=dev)[None, :] >= size[:, None]] = 0
+    pick = torch.rand(B, generator=gen, device=dev)
+    sub[pick >= 0.5] = -1
+    line = torch.randint(0, gm.n_line, (B,), generator=gen, device=dev, dtype=torch.int32)
+    line[(pick < 0.5) | (pick >= 0.8)] = -1
+    lst = torch.where(torch.rand(B, generator=gen, device=dev) < 0.5, -1, 1).to(torch.int32)
+    return sub, bus, line, lst
+
+
+def run(name, B, protections, steps, warmup, repeats):
+    import torch
+    from conftest import env_grid
+    from grid2op_b200.batched_env import BatchedEnv
+    from grid2op_b200.chronics import list_scenarios, load_scenarios
+    from grid2op_b200.gridmodel import GridModel
+    grid = env_grid(name)
+    gm = GridModel(grid)
+    env_dir = os.path.dirname(grid)
+    folders = list_scenarios(os.path.join(env_dir, "chronics"))[:4]
+    chron = load_scenarios(os.path.join(env_dir, "chronics"), gm, scenarios=folders)
+    dev = torch.device("cuda", 0)
+    envs = {}
+    for mode in ("host", "tensor"):
+        e = BatchedEnv(gm, chron, B, nb_timestep_cooldown_line=2, nb_timestep_cooldown_sub=2, protections=protections)
+        e.enable_observation(env_dir, scenarios=folders)
+        if protections:             # (random actions reach more new topologies per step than the automatic policy plans for)
+            e.engine.set_kernel_policy(e.engine.KERNEL_PLANNED)
+        envs[mode] = e
+    gens = {m: torch.Generator(device=dev) for m in envs}
+    for m, g in gens.items():
+        g.manual_seed(0)
+
+    def one(mode):
+        e = envs[mode]
+        sub, bus, line, lst = draw(e, gens[mode], dev)
+        if mode == "host":
+            _, done, _ = e.step(sub.cpu().numpy(), bus.cpu().numpy(), line.cpu().numpy(), lst.cpu().numpy())
+            e.observe()
+            if done.any():                                    # finished instances restart
+                e.reset_instances(np.flatnonzero(done))
+        else:
+            _, done, _ = e.step_tensors(sub, bus, line, lst)
+            e.observe()
+            e.reset_instances(done.clone())
+
+    topo_up = [0]
+    orig = envs["host"].engine.series_set_topo
+
+    def set_topo(topo):
+        topo_up[0] += 1
+        return orig(topo)
+    envs["host"].engine.series_set_topo = set_topo
+
+    def timed(mode):
+        for _ in range(warmup):
+            one(mode)
+        torch.cuda.synchronize()
+        s0 = envs[mode].engine.env_stats() if mode == "tensor" else None
+        o0 = envs[mode].engine.obs_stats()
+        topo_up[0] = 0
+        t0 = time.perf_counter()
+        for _ in range(steps):
+            one(mode)
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+        o1 = envs[mode].engine.obs_stats()
+        if mode == "tensor":
+            s1 = envs[mode].engine.env_stats()
+            h2d, d2h = s1["h2d_bytes"] - s0["h2d_bytes"], s1["d2h_bytes"] - s0["d2h_bytes"] + o1["d2h_bytes"] - o0["d2h_bytes"]
+        else:                      # observe inputs + series fetches; the topology uploads are added below
+            h2d, d2h = o1["h2d_bytes"] - o0["h2d_bytes"], o1["d2h_bytes"] - o0["d2h_bytes"]
+            h2d += topo_up[0] * envs[mode].gm.n_topo_in * B
+            topo_up[0] = 0
+        return B * steps / dt, h2d / steps, d2h / steps
+
+    res = {m: [] for m in envs}
+    envs["host"].reset_step(); envs["tensor"].step_tensors(from_reset=True)
+    for _ in range(repeats):
+        for m in ("host", "tensor"):
+            res[m].append(timed(m))
+    for m in ("host", "tensor"):
+        r = np.array([x[0] for x in res[m]])
+        print(f"{name:28s} B={B:5d} prot={int(protections)} {m:6s}: env.step/s min {r.min():.3e} median {np.median(r):.3e} max {r.max():.3e}; "
+              f"per step H2D {res[m][-1][1] / 1e3:.1f} kB, "
+              f"D2H {res[m][-1][2] / 1e3:.1f} kB")
+    for e in envs.values():
+        e.close()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--repeats", type=int, default=5)
+    args = ap.parse_args()
+    print("card, power limit:", card())
+    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024)):
+        for prot in (False, True):
+            run(name, B, prot, args.steps, args.warmup, args.repeats)
+
+
+if __name__ == "__main__":
+    main()
