@@ -112,6 +112,7 @@ class BatchedEnv(BatchedDoNothing):
         # "device"); a host-path call pulls it, the next step_tensors pushes it back
         self._dev = None
         self._authority = "host"
+        self._opp = None                                                   # line-attack opponent (:meth:`enable_opponent`)
 
     # ------------------------------------------------------------------------------------------------------------
     def _bus_cap(self) -> int:
@@ -273,9 +274,14 @@ class BatchedEnv(BatchedDoNothing):
         device (:meth:`fetch`)."""
         self._to_host()
         gm = self.gm
+        opp = None
+        if self._opp is not None:             # the opponent decides on the line status and rho the previous step left
+            opp = self._opponent_decide(from_reset)
         aff_l, aff_s = self._apply_agent(sub_id, sub_bus, line_id, line_status) if not from_reset else (
             np.zeros((self.batch, gm.n_line), dtype=bool), np.zeros((self.batch, gm.n_sub), dtype=bool))
         self._apply_environment()
+        if opp is not None:                   # its attack lands after the agent's action and the environment's outages
+            self._apply_attack(*opp)
         if self._topo_dirty:
             self.engine.series_set_topo(self.topo)
             self._topo_dirty = False
@@ -332,8 +338,68 @@ class BatchedEnv(BatchedDoNothing):
                 self._obs["reset"][live] = True
         else:
             self.current_step[live] += 1
-        return rho, self.done.copy(), {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done,
-                                       "is_illegal": self.is_illegal.copy()}
+        info = {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done, "is_illegal": self.is_illegal.copy()}
+        if opp is not None:
+            info["opponent_attack_line"], info["opponent_attack_duration"] = opp
+        return rho, self.done.copy(), info
+
+    # ---- line-attack opponent ---------------------------------------------------------------------------------------------
+    def enable_opponent(self, kind: str, lines_attacked, *, attack_duration: int, attack_cooldown: int, budget_per_ts: float,
+                        init_budget: float, attack_period: Optional[int] = None, rho_normalization=None, seeds):
+        """Give every instance grid2op's line-attack opponent (``OpponentSpace`` + ``BaseActionBudget``): ``kind``
+        ``"RandomLineOpponent"`` or ``"WeightedRandomOpponent"``; ``lines_attacked``: line names (``GridModel.name_line``) or ids;
+        the other parameters are the environment config's ``opponent_attack_duration``, ``opponent_attack_cooldown``,
+        ``opponent_budget_per_ts``, ``opponent_init_budget`` and ``kwargs_opponent`` (``attack_period``, ``rho_normalization``);
+        ``seeds``: int [B], the opponent seed of each instance (:func:`grid2op_b200.opponent.opponent_seed` of an environment
+        seed gives the one ``env.seed`` gives).  Every instance starts from ``OpponentSpace.reset()``; :meth:`reset_instances`
+        resets it again (its random stream continues).  Call it after the first step (``reset_step``): the weighted opponent reads
+        the rho of the previous step.  From then on :meth:`step` / :meth:`step_tensors` report ``info["opponent_attack_line"]``
+        (int32 [B], -1: none) and ``info["opponent_attack_duration"]`` (int32 [B])."""
+        from .opponent import BatchedOpponent
+        if self.n_steps == 0:
+            raise RuntimeError("enable_opponent() after the first step (reset_step): the opponent observes the previous step")
+        self._to_host()
+        names = list(getattr(self.gm, "name_line", []))
+        ids = [names.index(x) if isinstance(x, str) else int(x) for x in lines_attacked]
+        if any(not 0 <= l < self.gm.n_line for l in ids):
+            raise ValueError("attacked line out of range")
+        self._opp = BatchedOpponent(kind, ids, self.batch, attack_duration=attack_duration, attack_cooldown=attack_cooldown,
+                                    budget_per_ts=budget_per_ts, init_budget=init_budget, seeds=seeds, attack_period=attack_period,
+                                    rho_normalization=rho_normalization)
+        if self._dev is not None:
+            self._opp_bind_device()
+
+    def _opponent_decide(self, from_reset):
+        """OpponentSpace.attack of the live instances (none on a reset step) -> (line int32 [B], duration int32 [B])"""
+        o = self._opp
+        if from_reset:
+            return np.full(self.batch, -1, dtype=np.int32), np.zeros(self.batch, dtype=np.int32)
+        rho = self.engine.series_fetch(want_out=False)[3] if o.weighted else None        # (what the previous step wrote)
+        return o.attack(self.line_status(), rho, ~self.done)
+
+    def _apply_attack(self, line, dur):
+        """the attacked lines are out (both ends), their cooldown at least the attack's duration"""
+        ii = np.flatnonzero(line >= 0)
+        if not len(ii):
+            return
+        ll = line[ii].astype(np.int64)
+        lc = self.line_cooldown
+        lc[ii, ll] = np.maximum(lc[ii, ll], dur[ii])
+        was_on = (self.topo[ii, self.line_or_pos[ll]] > 0) | (self.topo[ii, self.line_ex_pos[ll]] > 0)
+        self.topo[ii, self.line_or_pos[ll]] = -1
+        self.topo[ii, self.line_ex_pos[ll]] = -1
+        if was_on.any():
+            self._topo_dirty = True
+            self._cap_dirty[ii[was_on]] = True
+
+    def opponent_state(self) -> dict:
+        """the opponent state of every instance as the device keeps it: budget float64 [B], budget64 uint8 [B] (the budget is a
+        float64 since its first charge), ctr int32 [B, 4] (attack duration, cooldown, last line, steps to the weighted opponent's
+        next attack), mt uint32 [B, 624] / mt_pos int32 [B] (the random streams)"""
+        if self._opp is None:
+            raise RuntimeError("call enable_opponent() first")
+        self._to_host()
+        return self._opp.get_state()
 
     def line_angles(self, out: np.ndarray):
         """``theta_or, theta_ex`` [B, n_line] of the full result records ``out`` (:meth:`fetch`) as an OBSERVATION of the reference
@@ -387,6 +453,8 @@ class BatchedEnv(BatchedDoNothing):
         if self._obs is not None:
             self._obs["reset"][idx] = True
         self.row[idx] = rows
+        if self._opp is not None:
+            self._opp.reset(idx)
         self.engine.series_reset_instances(idx, t_new=rows % self.chron.shape[1], topo_rows=self.topo[idx])
         self._cap_dirty[idx] = True
         if self.tight_cap:
@@ -519,7 +587,22 @@ class BatchedEnv(BatchedDoNothing):
         st["device"] = dev
         self._dev = st
         self._illegal_seen = 0
+        if self._opp is not None:
+            self._opp_bind_device()
         return st
+
+    def _opp_bind_device(self):
+        """the opponent's constants and initial random states to the device; its per-step outputs are device buffers of ours"""
+        import torch
+        d, o, B = self._dev, self._opp, self.batch
+        z = lambda dt: torch.zeros(B, dtype=dt, device=d["device"])           # noqa: E731
+        d["opp_line"], d["opp_dur"], d["opp_budget"] = z(torch.int32), z(torch.int32), z(torch.float64)
+        s = o.get_state()
+        self.engine.opp_bind(dict(kind=o.code, lines=o.lines, rho_norm=o.rho_norm, attack_period=o.attack_period,
+                                  attack_duration=int(o.attack_duration), attack_cooldown=int(o.attack_cooldown),
+                                  budget_per_ts=float(o.budget_per_ts), init_budget=float(o.init_budget), mt=s["mt"], mt_pos=s["mt_pos"]),
+                             d["opp_line"].data_ptr(), d["opp_dur"].data_ptr(), d["opp_budget"].data_ptr())
+        self._authority = "host"              # (the next step_tensors pushes the whole state, the opponent's included)
 
     def _to_device(self):
         """hand the host state to the tensor path"""
@@ -534,6 +617,8 @@ class BatchedEnv(BatchedDoNothing):
         obs = self._obs is not None
         self.engine.env_set_state(self.topo, self._nb_inst, self._cap_dirty, self._obs["reset"] if obs else None,
                                   self.observe_inputs() if obs else None)
+        if self._opp is not None:
+            self.engine.opp_set_state(self._opp.get_state())
         self._illegal_seen = self.engine.env_stats()["n_illegal"]
         self._authority = "device"
 
@@ -552,6 +637,8 @@ class BatchedEnv(BatchedDoNothing):
         self._nb_inst[:] = s["nb_inst"]; self._cap_dirty[:] = s["cap_dirty"]
         if self._obs is not None:
             self._obs["reset"][:] = s["obs_reset"]
+        if self._opp is not None:
+            self._opp.set_state(self.engine.opp_get_state())
         if self.tight_cap and self._cap_dirty.any():
             self.nb_cap = self._bus_cap()
 
@@ -615,6 +702,8 @@ class BatchedEnv(BatchedDoNothing):
             self.nb_cap = st["nb_cap"]
         info = {"status": d["status"], "iters": d["iters"], "newly_done": d["newly_done"], "is_illegal": d["is_illegal"],
                 "disc_lines": d["disc"] if self.protections else None}
+        if self._opp is not None:
+            info["opponent_attack_line"], info["opponent_attack_duration"] = d["opp_line"], d["opp_dur"]
         return d["rho"], d["done"], info
 
     def _reset_tensors(self, mask, rows=None):

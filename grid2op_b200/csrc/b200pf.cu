@@ -121,6 +121,9 @@ struct b200pf_handle {
     std::vector<int8_t> env_topo0; std::vector<uint8_t> env_mask;   // host copies: reset topologies, the last reset mask
     int64_t env_steps = 0, env_h2d = 0, env_d2h = 0, env_waits = 0, env_illegal = 0, env_plan_refresh = 0;
     int env_last_cap = 0, env_last_dirty = 0;
+    // line-attack opponent of the device environment (b200pf_opp_bind)
+    OppArgs opp{}; int opp_batch = 0;
+    std::vector<void *> opp_allocs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -331,6 +334,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     if (h->obs_ev) cudaEventDestroy(h->obs_ev);
     for (void *p : h->env_allocs) cudaFree(p);
     if (h->h_env_ctl) cudaFreeHost(h->h_env_ctl);
+    for (void *p : h->opp_allocs) cudaFree(p);
     delete h;
     return 0;
 }
@@ -1939,6 +1943,14 @@ extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
 
 static inline unsigned env_grid(int n) { return (unsigned)((n + 127) / 128); }
 
+// the opponent the env launches run: the bound one, or none (kind OPP_NONE)
+static OppArgs env_opp(const b200pf_handle *h) {
+    if (!h->opp_batch || h->opp_batch != h->env_batch) return OppArgs{};
+    OppArgs o = h->opp;
+    o.rho = h->x_rho ? h->x_rho : h->d_rho;                  // what the previous step wrote
+    return o;
+}
+
 extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
                                const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter,
                                double tol_mva, int tight_cap, int stamp) {
@@ -1961,7 +1973,7 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
         pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a);
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h));
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2025,7 +2037,7 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     a.reset_mask = d_mask; a.reset_rows = d_rows;
     const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
     a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a);
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h));
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2120,6 +2132,92 @@ extern "C" int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_re
     pf_kernel_env_observed<<<env_grid(e.batch), 128, 0, h->stream>>>(e);
     CU(cudaGetLastError());
     h->obs_launches++;
+    return 0;
+}
+
+extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    const DevGrid &g = h->g;
+    if ((d->kind != OPP_RANDOM_LINE && d->kind != OPP_WEIGHTED_RANDOM) || d->n_attack < 1 || d->n_attack > OPP_MAX_ATTACK || !d->lines ||
+        (d->kind == OPP_WEIGHTED_RANDOM && (!d->rho_norm || d->attack_period < 1)) || d->attack_duration < 0 || d->attack_cooldown < 0 ||
+        !d->mt || !d->mt_pos || !d->attack_line || !d->attack_dur || !d->budget)
+        return fail(B200PF_E_ARG, "bad opponent description");
+    for (int k = 0; k < d->n_attack; ++k) if (d->lines[k] < 0 || d->lines[k] >= g.n_line) return fail(B200PF_E_ARG, "attacked line out of range");
+    const int B = h->env_batch;
+    for (int i = 0; i < B; ++i) if (d->mt_pos[i] < 0 || d->mt_pos[i] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (void *p : h->opp_allocs) cudaFree(p);
+    h->opp_allocs.clear();
+    h->opp_batch = 0;
+    auto dev = [&](const void *src, size_t bytes, void **dst) -> int {
+        CU(cudaMalloc(dst, bytes));
+        h->opp_allocs.push_back(*dst);
+        if (src) H2D(*dst, src, bytes);
+        return 0;
+    };
+    void *p[6] = {};
+    int rc;
+    if ((rc = dev(d->lines, (size_t)d->n_attack * 4, &p[0])) ||
+        (rc = dev(d->rho_norm, (size_t)d->n_attack * 8, &p[1])) || (rc = dev(nullptr, (size_t)B, &p[2])) ||
+        (rc = dev(nullptr, (size_t)B * OPP_CTR * 4, &p[3])) || (rc = dev(d->mt, (size_t)B * OPP_MT_N * 4, &p[4])) ||
+        (rc = dev(d->mt_pos, (size_t)B * 4, &p[5])))
+        return rc;
+    OppArgs o{};
+    o.kind = d->kind; o.n_attack = d->n_attack; o.lines = (const int32_t *)p[0]; o.rho_norm = (const double *)p[1];
+    o.attack_period = d->attack_period; o.attack_duration = d->attack_duration; o.attack_cooldown = d->attack_cooldown;
+    o.budget_per_ts = d->budget_per_ts; o.init_budget = d->init_budget;
+    o.budget = d->budget; o.budget64 = (uint8_t *)p[2]; o.ctr = (int32_t *)p[3]; o.mt = (uint32_t *)p[4]; o.mt_pos = (int32_t *)p[5];
+    o.attack_line = d->attack_line; o.attack_dur = d->attack_dur;
+    // every instance starts from OpponentSpace.reset()
+    std::vector<double> bud((size_t)B, (double)d->init_budget);
+    std::vector<int32_t> ctr((size_t)B * OPP_CTR);
+    for (int i = 0; i < B; ++i) {
+        ctr[(size_t)i * OPP_CTR + OPP_CTR_DURATION] = 0; ctr[(size_t)i * OPP_CTR + OPP_CTR_COOLDOWN] = d->attack_cooldown;
+        ctr[(size_t)i * OPP_CTR + OPP_CTR_LAST] = -1; ctr[(size_t)i * OPP_CTR + OPP_CTR_NEXT] = OPP_NEXT_UNSET;
+    }
+    H2D(o.budget, bud.data(), (size_t)B * 8);
+    H2D(o.ctr, ctr.data(), ctr.size() * 4);
+    CU(cudaMemsetAsync(o.budget64, 0, (size_t)B, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->opp = o; h->opp_batch = B;
+    return 0;
+}
+
+static bool opp_bound(const b200pf_handle *h) { return env_bound(h) && h->opp_batch == h->env_batch; }
+
+extern "C" int b200pf_opp_get_state(b200pf_handle *h, double *budget, uint8_t *budget64, int32_t *ctr, uint32_t *mt, int32_t *mt_pos) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_bound(h)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
+    CU(cudaSetDevice(h->device));
+    const size_t B = (size_t)h->opp_batch;
+    const OppArgs &o = h->opp;
+    CU(cudaStreamSynchronize(h->stream));
+    if (budget) CU(cudaMemcpy(budget, o.budget, B * 8, cudaMemcpyDeviceToHost));
+    if (budget64) CU(cudaMemcpy(budget64, o.budget64, B, cudaMemcpyDeviceToHost));
+    if (ctr) CU(cudaMemcpy(ctr, o.ctr, B * OPP_CTR * 4, cudaMemcpyDeviceToHost));
+    if (mt) CU(cudaMemcpy(mt, o.mt, B * OPP_MT_N * 4, cudaMemcpyDeviceToHost));
+    if (mt_pos) CU(cudaMemcpy(mt_pos, o.mt_pos, B * 4, cudaMemcpyDeviceToHost));
+    h->env_d2h += (int64_t)((budget ? B * 8 : 0) + (budget64 ? B : 0) + (ctr ? B * OPP_CTR * 4 : 0) + (mt ? B * OPP_MT_N * 4 : 0) + (mt_pos ? B * 4 : 0));
+    return 0;
+}
+
+extern "C" int b200pf_opp_set_state(b200pf_handle *h, const double *budget, const uint8_t *budget64, const int32_t *ctr, const uint32_t *mt,
+                                    const int32_t *mt_pos) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_bound(h)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
+    const size_t B = (size_t)h->opp_batch;
+    if (mt_pos) for (size_t i = 0; i < B; ++i) if (mt_pos[i] < 0 || mt_pos[i] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
+    CU(cudaSetDevice(h->device));
+    const OppArgs &o = h->opp;
+    if (budget) H2D(o.budget, budget, B * 8);
+    if (budget64) H2D(o.budget64, budget64, B);
+    if (ctr) H2D(o.ctr, ctr, B * OPP_CTR * 4);
+    if (mt) H2D(o.mt, mt, B * OPP_MT_N * 4);
+    if (mt_pos) H2D(o.mt_pos, mt_pos, B * 4);
+    CU(cudaStreamSynchronize(h->stream));
+    h->env_h2d += (int64_t)((budget ? B * 8 : 0) + (budget64 ? B : 0) + (ctr ? B * OPP_CTR * 4 : 0) + (mt ? B * OPP_MT_N * 4 : 0) + (mt_pos ? B * 4 : 0));
     return 0;
 }
 

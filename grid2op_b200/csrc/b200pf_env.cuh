@@ -3,15 +3,19 @@
 // isolated-busbar rule, cooldowns, game over, the observe layer's per-instance input record).
 //
 // Every body restates, per instance, the numpy code of grid2op_b200/batched_env.py in the same order:
-//   env_apply_instance   BatchedEnv._apply_agent, then _apply_environment (and the bus count of _bus_cap);
+//   env_apply_instance   BatchedEnv._apply_agent, then _apply_environment (and the bus count of _bus_cap), with the opponent's
+//                        decision before the agent's action and its attack after the outages when one is bound (b200pf_opp.cuh);
 //   env_post_instance    the rest of BatchedEnv.step behind the solve;
-//   env_reset_instance   BatchedEnv.reset_instances (with the library's part, b200pf_series_reset_instances).
-// The bodies are __host__ __device__: the CUDA launches run one thread per instance, a host build (tests/emu/env_emu.cpp) runs
-// the same source over the batch.  Only integer arithmetic: the two builds are bit-identical by construction.
+//   env_reset_instance   BatchedEnv.reset_instances (with the library's part, b200pf_series_reset_instances, and the opponent's).
+// The bodies are __host__ __device__: the CUDA launches run one thread per instance, a host build (tests/emu/env_emu.cpp,
+// tests/emu/opp_emu.cpp) runs the same source over the batch.  Integer arithmetic, and the opponent's fp64 operations explicitly
+// rounded: the two builds are bit-identical by construction.
 #pragma once
 
 #include <cstddef>
 #include <cstdint>
+
+#include "b200pf_opp.cuh"
 
 #if defined(__CUDACC__)
 #define ENV_HD __host__ __device__
@@ -118,8 +122,8 @@ ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
     return n;
 }
 
-// BatchedEnv._apply_agent followed by _apply_environment, for instance i
-ENV_HD inline void env_apply_instance(const EnvArgs &a, int i) {
+// BatchedEnv._apply_agent followed by _apply_environment and the opponent's attack (o: NULL or no opponent bound), for instance i
+ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr) {
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * a.dim_topo;
@@ -129,6 +133,12 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i) {
     a.aff_s[i] = -1;
     const bool done = a.done[i] != 0;
     bool dirty = false;
+    // the opponent decides first, on the line status the previous step left (grid2op's current_obs); its attack lands last
+    int opp_line = -1, opp_dur = 0;
+    if (o && o->kind != OPP_NONE) {
+        if (!done && !a.from_reset) opp_line = opp_decide_instance(*o, i, tv, a.line_or_pos, a.line_ex_pos, nl, &opp_dur);
+        o->attack_line[i] = opp_line; o->attack_dur[i] = opp_dur;
+    }
     if (!a.from_reset) {
         bool has_sub = false, has_line = false;
         int sid = -1, lid = -1, lst = 0;
@@ -222,6 +232,13 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i) {
             tv[po] = -1; tv[pe] = -1;
         }
     }
+    if (opp_line >= 0) {                                      // the attack: the line is out, its cooldown at least the attack's duration
+        int32_t *lc = a.line_cd + (size_t)i * nl;
+        if (lc[opp_line] < opp_dur) lc[opp_line] = opp_dur;
+        const int po = a.line_or_pos[opp_line], pe = a.line_ex_pos[opp_line];
+        if (tv[po] > 0 || tv[pe] > 0) dirty = true;
+        tv[po] = -1; tv[pe] = -1;
+    }
     if (dirty) { a.cap_dirty[i] = 1; ENV_ATOMIC_ADD(&a.ctl[ENV_CTL_N_DIRTY], 1); }
     if (dirty || a.stale[i]) {                                // rows the host's plan mirror has not seen
         const int k = ENV_ATOMIC_ADD(&a.ctl[ENV_CTL_N_COPY], 1);
@@ -302,9 +319,10 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i) {
     }
 }
 
-// BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0)
-ENV_HD inline void env_reset_instance(const EnvArgs &a, int i) {
+// BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
+ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr) {
     if (!a.reset_mask[i]) return;
+    if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const int8_t *t0v = a.topo0 + (size_t)i * a.n_topo_in;
@@ -347,10 +365,10 @@ __global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a) {
 }
 
 // one thread per instance; nothing is written when the validation flagged an input
-__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a) {
+__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.batch || *(volatile int32_t *)&a.ctl[ENV_CTL_ERR]) return;
-    env_apply_instance(a, i);
+    env_apply_instance(a, i, &o);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
@@ -358,9 +376,9 @@ __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
     if (i < a.batch) env_post_instance(a, i);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_reset_instance(a, i);
+    if (i < a.batch) env_reset_instance(a, i, &o);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

@@ -1,0 +1,203 @@
+// b200pf_opp.cuh — line-attack opponents of BatchedEnv for a whole batch on the device: grid2op's OpponentSpace with
+// BaseActionBudget and a RandomLineOpponent or a WeightedRandomOpponent, restated per instance, with each instance's own
+// numpy-legacy random stream (RandomState: MT19937 and its legacy draws).
+//
+// The body restates grid2op_b200/opponent.py (the numpy reference path) in the same order:
+//   opp_decide_instance   OpponentSpace.attack and the opponent's attack / tell_attack_continues, on the line status and rho
+//                         the previous step left;
+//   opp_reset_instance    OpponentSpace.reset (the random stream is not reseeded: it continues).
+// env_apply_instance (b200pf_env.cuh) calls the first before the agent's action and applies the attack after the environment's
+// own outages; env_reset_instance calls the second.  The bodies are __host__ __device__: the CUDA launches run one thread per
+// instance, a host build (tests/emu/opp_emu.cpp) runs the same source over the batch.  The fp64 arithmetic of the weighted draw is
+// written with explicitly rounded operations (no contraction), so both builds round as numpy does.
+#pragma once
+
+#include <cstddef>
+#include <cstdint>
+
+#if defined(__CUDACC__)
+#define OPP_HD __host__ __device__
+#else
+#define OPP_HD
+#endif
+
+namespace b200pf {
+
+enum { OPP_NONE = 0, OPP_RANDOM_LINE = 1, OPP_WEIGHTED_RANDOM = 2 };
+enum { OPP_MT_N = 624, OPP_MAX_ATTACK = 64 };
+// per-instance counters, int32 [batch][OPP_CTR]
+enum { OPP_CTR_DURATION = 0, OPP_CTR_COOLDOWN = 1, OPP_CTR_LAST = 2, OPP_CTR_NEXT = 3, OPP_CTR = 4 };
+static const int32_t OPP_NEXT_UNSET = INT32_MIN;    // WeightedRandomOpponent._next_attack_time is None
+
+struct OppArgs {
+    int kind;                                       // OPP_NONE: no opponent bound
+    int n_attack;                                   // attackable lines
+    const int32_t *lines;                           // [n_attack] their line ids
+    const double *rho_norm;                         // [n_attack] (weighted)
+    int attack_period, attack_duration, attack_cooldown;
+    float budget_per_ts, init_budget;
+    // per-instance state
+    double *budget;                                 // [batch] caller-owned; float32 value until the first charge (budget64)
+    uint8_t *budget64;                              // [batch] the budget has become a float64 (numpy promotion)
+    int32_t *ctr;                                   // [batch][OPP_CTR]
+    uint32_t *mt; int32_t *mt_pos;                  // [batch][624], [batch]: MT19937 state as RandomState.get_state() gives it
+    // per-step outputs, caller-owned [batch]
+    int32_t *attack_line, *attack_dur;
+    // the previous step's rho [batch][n_line] (read by the weighted opponent)
+    const float *rho;
+};
+
+// ---- numpy legacy RandomState draws --------------------------------------------------------------------------------------
+OPP_HD inline uint32_t opp_next_u32(uint32_t *mt, int32_t *pos) {
+    if (*pos >= OPP_MT_N) {                                   // the twist (mt19937_gen)
+        int k = 0;
+        for (; k < OPP_MT_N - 397; ++k) {
+            const uint32_t y = (mt[k] & 0x80000000u) | (mt[k + 1] & 0x7fffffffu);
+            mt[k] = mt[k + 397] ^ (y >> 1) ^ ((0u - (y & 1u)) & 0x9908b0dfu);
+        }
+        for (; k < OPP_MT_N - 1; ++k) {
+            const uint32_t y = (mt[k] & 0x80000000u) | (mt[k + 1] & 0x7fffffffu);
+            mt[k] = mt[k + (397 - OPP_MT_N)] ^ (y >> 1) ^ ((0u - (y & 1u)) & 0x9908b0dfu);
+        }
+        const uint32_t y = (mt[OPP_MT_N - 1] & 0x80000000u) | (mt[0] & 0x7fffffffu);
+        mt[OPP_MT_N - 1] = mt[396] ^ (y >> 1) ^ ((0u - (y & 1u)) & 0x9908b0dfu);
+        *pos = 0;
+    }
+    uint32_t y = mt[(*pos)++];
+    y ^= y >> 11;
+    y ^= (y << 7) & 0x9d2c5680u;
+    y ^= (y << 15) & 0xefc60000u;
+    y ^= y >> 18;
+    return y;
+}
+
+// randint(n) / choice(n) without p, n <= 2**32: masked rejection on 32-bit words; n == 1 draws nothing
+OPP_HD inline uint32_t opp_randint(uint32_t *mt, int32_t *pos, uint32_t n) {
+    const uint32_t rng = n - 1u;
+    if (rng == 0u) return 0u;
+    uint32_t mask = rng;
+    mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
+    uint32_t w;
+    while ((w = opp_next_u32(mt, pos) & mask) > rng) {}
+    return w;
+}
+
+OPP_HD inline double opp_dmul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+OPP_HD inline double opp_dadd(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+OPP_HD inline double opp_ddiv(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+
+// random_sample(): 53 bits from two words
+OPP_HD inline double opp_random_sample(uint32_t *mt, int32_t *pos) {
+    const uint32_t a = opp_next_u32(mt, pos) >> 5, b = opp_next_u32(mt, pos) >> 6;
+    return opp_ddiv(opp_dadd(opp_dmul((double)a, 67108864.0), (double)b), 9007199254740992.0);
+}
+
+// ndarray.sum() of n float64 values: numpy's pairwise summation (one block below 128 values)
+OPP_HD inline double opp_np_sum(const double *v, int n) {
+    if (n < 8) {
+        double s = 0.0;
+        for (int k = 0; k < n; ++k) s = opp_dadd(s, v[k]);
+        return s;
+    }
+    double r[8];
+    for (int j = 0; j < 8; ++j) r[j] = v[j];
+    int k = 8;
+    for (; k < n - (n % 8); k += 8)
+        for (int j = 0; j < 8; ++j) r[j] = opp_dadd(r[j], v[k + j]);
+    double s = opp_dadd(opp_dadd(opp_dadd(r[0], r[1]), opp_dadd(r[2], r[3])), opp_dadd(opp_dadd(r[4], r[5]), opp_dadd(r[6], r[7])));
+    for (; k < n; ++k) s = opp_dadd(s, v[k]);
+    return s;
+}
+
+// choice(n, p=w / w.sum()) for w >= 0 with a positive sum: cdf = cumsum(p), cdf /= cdf[-1], searchsorted(cdf, random_sample(), "right")
+OPP_HD inline int opp_choice_weighted(uint32_t *mt, int32_t *pos, const double *w, int n, double wsum) {
+    double cdf[OPP_MAX_ATTACK];
+    double c = 0.0;
+    for (int k = 0; k < n; ++k) { c = opp_dadd(c, opp_ddiv(w[k], wsum)); cdf[k] = c; }
+    const double last = cdf[n - 1];
+    const double u = opp_random_sample(mt, pos);
+    int idx = 0;
+    for (int k = 0; k < n; ++k) idx += opp_ddiv(cdf[k], last) <= u ? 1 : 0;
+    return idx;
+}
+
+// ---- the opponent ---------------------------------------------------------------------------------------------------------
+// The opponent's choice among the attackable lines that are connected in ``tv`` (the topology the previous step left): -1 for none.
+OPP_HD inline int opp_choose(const OppArgs &o, int i, const int8_t *tv, const int32_t *line_or_pos, const int32_t *line_ex_pos,
+                             int n_line, int32_t *ctr) {
+    uint32_t *mt = o.mt + (size_t)i * OPP_MT_N;
+    int32_t *pos = o.mt_pos + i;
+    int on[OPP_MAX_ATTACK];
+    int n_on = 0;
+    if (o.kind == OPP_WEIGHTED_RANDOM) {
+        if (ctr[OPP_CTR_NEXT] == OPP_NEXT_UNSET) ctr[OPP_CTR_NEXT] = 1 + (int32_t)opp_randint(mt, pos, (uint32_t)o.attack_period);
+        ctr[OPP_CTR_NEXT] -= 1;
+        if (ctr[OPP_CTR_NEXT] > 0) return -1;
+    }
+    for (int k = 0; k < o.n_attack; ++k) {
+        const int l = o.lines[k];
+        if (tv[line_or_pos[l]] > 0 && tv[line_ex_pos[l]] > 0) on[n_on++] = k;
+    }
+    if (n_on == 0) return -1;
+    if (o.kind == OPP_RANDOM_LINE) return o.lines[on[opp_randint(mt, pos, (uint32_t)n_on)]];
+    double w[OPP_MAX_ATTACK];
+    const float *rho = o.rho + (size_t)i * n_line;
+    for (int k = 0; k < n_on; ++k) w[k] = opp_ddiv((double)rho[o.lines[on[k]]], o.rho_norm[on[k]]);
+    const double s = opp_np_sum(w, n_on);
+    if (!(s > 0.0)) return -1;
+    return o.lines[on[opp_choice_weighted(mt, pos, w, n_on, s)]];
+}
+
+// OpponentSpace.attack for instance i (not finished, not a reset step) -> the attacked line (-1: none); *dur: its duration
+OPP_HD inline int opp_decide_instance(const OppArgs &o, int i, const int8_t *tv, const int32_t *line_or_pos, const int32_t *line_ex_pos,
+                                      int n_line, int *dur) {
+    int32_t *ctr = o.ctr + (size_t)i * OPP_CTR;
+    double b = o.budget[i];
+    const bool b64 = o.budget64[i] != 0;
+    b = b64 ? b + (double)o.budget_per_ts : (double)((float)b + o.budget_per_ts);      // budget += budget_per_timestep
+    ctr[OPP_CTR_DURATION] = ctr[OPP_CTR_DURATION] > 1 ? ctr[OPP_CTR_DURATION] - 1 : 0;
+    ctr[OPP_CTR_COOLDOWN] = ctr[OPP_CTR_COOLDOWN] > 1 ? ctr[OPP_CTR_COOLDOWN] - 1 : 0;
+    int attack = -1;
+    bool asked = false;
+    if (ctr[OPP_CTR_DURATION] > 0) attack = ctr[OPP_CTR_LAST];                           // the running attack continues
+    else if (ctr[OPP_CTR_COOLDOWN] <= o.attack_cooldown) {
+        asked = true;
+        attack = opp_choose(o, i, tv, line_or_pos, line_ex_pos, n_line, ctr);
+        // duration None -> attack_max_duration; the cost of one line is 1: refused when duration * cost > budget
+        if (attack >= 0 && (double)o.attack_duration > b) attack = -1;
+        if (attack >= 0) { ctr[OPP_CTR_DURATION] = o.attack_duration; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
+    }
+    if (!asked && o.kind == OPP_WEIGHTED_RANDOM) ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;      // tell_attack_continues
+    ctr[OPP_CTR_LAST] = attack;
+    if (attack >= 0) { b = b - 1.0; o.budget64[i] = 1; }                                    // budget -= cost: float32 - int64 -> float64
+    o.budget[i] = b;
+    *dur = attack >= 0 ? ctr[OPP_CTR_DURATION] : 0;
+    return attack;
+}
+
+// OpponentSpace.reset for instance i
+OPP_HD inline void opp_reset_instance(const OppArgs &o, int i) {
+    int32_t *ctr = o.ctr + (size_t)i * OPP_CTR;
+    o.budget[i] = (double)o.init_budget; o.budget64[i] = 0;
+    ctr[OPP_CTR_DURATION] = 0; ctr[OPP_CTR_COOLDOWN] = o.attack_cooldown; ctr[OPP_CTR_LAST] = -1; ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;
+}
+
+}  // namespace b200pf

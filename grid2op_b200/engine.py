@@ -39,6 +39,7 @@ ABI_SYMBOLS = (
     "b200pf_series_reset_instances", "b200pf_grid_max_active_buses", "b200pf_obs_bind", "b200pf_observe", "b200pf_obs_stats",
     "b200pf_last_launch_config", "b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state",
     "b200pf_env_set_state", "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats",
+    "b200pf_opp_bind", "b200pf_opp_get_state", "b200pf_opp_set_state",
 )
 
 
@@ -87,6 +88,15 @@ class EnvDesc(C.Structure):
         ("topo0", C.c_void_p), ("t0", C.c_void_p),
         ("last_bus", C.c_void_p), ("line_cd", C.c_void_p), ("sub_cd", C.c_void_p), ("done", C.c_void_p), ("is_illegal", C.c_void_p),
         ("newly_done", C.c_void_p), ("current_step", C.c_void_p), ("status", C.c_void_p),
+    ]
+
+
+class OppDesc(C.Structure):
+    """``b200pf_opp_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("kind", C.c_int32), ("n_attack", C.c_int32), ("lines", C.c_void_p), ("rho_norm", C.c_void_p), ("attack_period", C.c_int32),
+        ("attack_duration", C.c_int32), ("attack_cooldown", C.c_int32), ("budget_per_ts", C.c_float), ("init_budget", C.c_float),
+        ("mt", C.c_void_p), ("mt_pos", C.c_void_p), ("attack_line", C.c_void_p), ("attack_dur", C.c_void_p), ("budget", C.c_void_p),
     ]
 
 
@@ -247,8 +257,12 @@ def load_library():
     lib.b200pf_env_pointers.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.b200pf_observe_device.argtypes = [vp, vp, vp]
     lib.b200pf_env_stats.argtypes = [vp, C.POINTER(C.c_int64)]
+    lib.b200pf_opp_bind.argtypes = [vp, C.POINTER(OppDesc)]
+    lib.b200pf_opp_get_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.b200pf_opp_set_state.argtypes = [vp, vp, vp, vp, vp, vp]
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
-               "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats"):
+               "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
+               "b200pf_opp_set_state"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -707,6 +721,32 @@ class PowerFlowEngine:
         p = [C.c_void_p() for _ in range(3)]
         self._check(self.lib.b200pf_env_pointers(self.h, *[C.byref(x) for x in p]), "b200pf_env_pointers")
         return dict(topo=p[0].value, t=p[1].value, disc=p[2].value)
+
+    def opp_bind(self, t: dict, d_attack_line: int, d_attack_dur: int, d_budget: int):
+        """Line-attack opponent of the device environment (``b200pf_opp_bind``): constants and initial random states ``t`` (built
+        by BatchedEnv.enable_opponent), caller-owned device outputs int32 / int32 / float64 [batch]."""
+        keep = [np.ascontiguousarray(t["lines"], np.int32), np.ascontiguousarray(t["rho_norm"], np.float64),
+                np.ascontiguousarray(t["mt"], np.uint32), np.ascontiguousarray(t["mt_pos"], np.int32)]
+        d = OppDesc(kind=int(t["kind"]), n_attack=len(keep[0]), lines=keep[0].ctypes.data, rho_norm=keep[1].ctypes.data,
+                    attack_period=int(t["attack_period"]), attack_duration=int(t["attack_duration"]), attack_cooldown=int(t["attack_cooldown"]),
+                    budget_per_ts=float(t["budget_per_ts"]), init_budget=float(t["init_budget"]), mt=keep[2].ctypes.data,
+                    mt_pos=keep[3].ctypes.data, attack_line=int(d_attack_line), attack_dur=int(d_attack_dur), budget=int(d_budget))
+        self._check(self.lib.b200pf_opp_bind(self.h, C.byref(d)), "b200pf_opp_bind")
+        del keep
+
+    def opp_get_state(self):
+        """-> dict(budget float64 [B], budget64 uint8 [B], ctr int32 [B, 4], mt uint32 [B, 624], mt_pos int32 [B])"""
+        B = self._series_batch
+        s = dict(budget=np.empty(B, np.float64), budget64=np.empty(B, np.uint8), ctr=np.empty((B, 4), np.int32),
+                 mt=np.empty((B, 624), np.uint32), mt_pos=np.empty(B, np.int32))
+        self._check(self.lib.b200pf_opp_get_state(self.h, *[_ptr(s[k]) for k in ("budget", "budget64", "ctr", "mt", "mt_pos")]),
+                    "b200pf_opp_get_state")
+        return s
+
+    def opp_set_state(self, s: dict):
+        a = [np.ascontiguousarray(s[k], dt) for k, dt in (("budget", np.float64), ("budget64", np.uint8), ("ctr", np.int32),
+                                                            ("mt", np.uint32), ("mt_pos", np.int32))]
+        self._check(self.lib.b200pf_opp_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_set_state")
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")

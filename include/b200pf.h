@@ -389,6 +389,39 @@ int b200pf_env_pointers(b200pf_handle *h, int8_t **d_topo, int32_t **d_t, int32_
 int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_reward);
 int b200pf_env_stats(const b200pf_handle *h, int64_t *out8);
 
+/* Line-attack opponent of the device environment (csrc/b200pf_opp.cuh): grid2op's OpponentSpace with BaseActionBudget and a
+ * RandomLineOpponent (kind 1) or a WeightedRandomOpponent (kind 2), attacking one line at a time with set_line_status -1, each
+ * instance with its own numpy-legacy random stream (RandomState: MT19937 state of 624 words and a position, as get_state() gives
+ * them).  b200pf_opp_bind needs a bound environment (b200pf_env_bind); it copies the constants and the initial random states, and
+ * sets every instance to OpponentSpace.reset()'s state.  From then on the apply launch of b200pf_env_step runs the opponent of every
+ * live instance before the agent's action, on the line status and rho the previous step left, and takes the attacked line out after
+ * the environment's outages, with its line cooldown raised to the attack's duration; a reset step and a finished instance attack
+ * nothing and draw nothing.  b200pf_env_reset resets the opponent of the reset instances (the random stream continues).  After
+ * each b200pf_env_step the caller-owned device buffers hold: attack_line int32 [batch] (-1: none), attack_dur int32 [batch] (0: none)
+ * and budget float64 [batch] (the opponent's budget, which is also its state).  b200pf_opp_get_state / b200pf_opp_set_state: the
+ * opponent state to the host and back (any pointer may be NULL): budget float64 [batch], budget64 uint8 [batch] (the budget has been
+ * charged since the last reset: grid2op then holds it as a float64, before as a float32), ctr int32 [batch][4] (current attack
+ * duration, current attack cooldown, last attacked line or -1, steps to the weighted opponent's next attack or INT32_MIN for
+ * none), mt uint32 [batch][624] and mt_pos int32 [batch].  Unbound (b200pf_opp_bind never called), nothing of the above runs. */
+typedef struct b200pf_opp_desc {
+    int32_t kind;                       /* 1: RandomLineOpponent, 2: WeightedRandomOpponent */
+    int32_t n_attack;                   /* attackable lines, 1..64 */
+    const int32_t *lines;               /* [n_attack] their line ids */
+    const double *rho_norm;             /* [n_attack] rho normalisation (kind 2) */
+    int32_t attack_period;              /* kind 2: an attack is drawn uniformly within this many steps */
+    int32_t attack_duration, attack_cooldown;
+    float budget_per_ts, init_budget;
+    const uint32_t *mt;                 /* [batch][624] initial MT19937 states */
+    const int32_t *mt_pos;              /* [batch] their positions (0..624) */
+    /* caller-owned device buffers [batch] */
+    int32_t *attack_line, *attack_dur;
+    double *budget;
+} b200pf_opp_desc;
+int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *desc);
+int b200pf_opp_get_state(b200pf_handle *h, double *budget, uint8_t *budget64, int32_t *ctr, uint32_t *mt, int32_t *mt_pos);
+int b200pf_opp_set_state(b200pf_handle *h, const double *budget, const uint8_t *budget64, const int32_t *ctr, const uint32_t *mt,
+                         const int32_t *mt_pos);
+
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */
 uint64_t b200pf_stream(b200pf_handle *h);

@@ -1,0 +1,114 @@
+"""BatchedEnv.step_tensors with and without the line-attack opponent (enable_opponent), alternating in one process, on the workloads
+of scripts/bench_env_tensor.py: random one-substation and one-line actions drawn on the GPU with a seeded torch generator, then
+observe, finished instances reset on the device; protections off and on; case14 at batch 4096 (RandomLineOpponent on the lines of
+rte_case14_opponent) and l2rpn_neurips_2020_track1 at batch 1024 (its WeightedRandomOpponent).  The opponents use their environments'
+constants with a small initial budget, so that attacks run from the first steps on.  A host clock around K steps that end in a device
+synchronise, after warm-up.  Prints env.step/s (min / median / max over the repeats), the extra bytes per step the opponent moves, and
+the card and its power limit read in the same run.
+
+    python scripts/bench_opponent.py [--steps 50] [--warmup 5] [--repeats 5]
+"""
+import argparse
+import os
+import sys
+import time
+
+import numpy as np
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+sys.path.insert(0, os.path.join(REPO, "tests"))
+sys.path.insert(0, os.path.join(REPO, "scripts"))
+
+OPPONENTS = {
+    "l2rpn_case14_sandbox": dict(kind="RandomLineOpponent", lines=["1_3_3", "1_4_4", "3_6_15", "9_10_12", "11_12_13", "12_13_14"],
+                                 attack_duration=48, attack_cooldown=288, budget_per_ts=0.5, init_budget=48.0),
+    "l2rpn_neurips_2020_track1": dict(kind="WeightedRandomOpponent",
+                                      lines=["62_58_180", "62_63_160", "48_50_136", "48_53_141", "41_48_131", "39_41_121", "43_44_125",
+                                             "44_45_126", "34_35_110", "54_58_154"],
+                                      rho_normalization=[0.45, 0.45, 0.6, 0.35, 0.3, 0.2, 0.55, 0.3, 0.45, 0.55], attack_period=12,
+                                      attack_duration=48, attack_cooldown=288, budget_per_ts=0.16667, init_budget=48.0),
+}
+
+
+def run(name, B, protections, steps, warmup, repeats):
+    import torch
+    from bench_env_tensor import draw
+    from conftest import env_grid
+    from grid2op_b200.batched_env import BatchedEnv
+    from grid2op_b200.chronics import list_scenarios, load_scenarios
+    from grid2op_b200.gridmodel import GridModel
+    from grid2op_b200.opponent import opponent_seed
+    grid = env_grid(name)
+    gm = GridModel(grid)
+    env_dir = os.path.dirname(grid)
+    folders = list_scenarios(os.path.join(env_dir, "chronics"))[:4]
+    chron = load_scenarios(os.path.join(env_dir, "chronics"), gm, scenarios=folders)
+    dev = torch.device("cuda", 0)
+    envs = {}
+    for mode in ("off", "on"):
+        e = BatchedEnv(gm, chron, B, nb_timestep_cooldown_line=2, nb_timestep_cooldown_sub=2, protections=protections)
+        e.enable_observation(env_dir, scenarios=folders)
+        if protections:
+            e.engine.set_kernel_policy(e.engine.KERNEL_PLANNED)
+        e.step_tensors(from_reset=True)
+        if mode == "on":
+            o = dict(OPPONENTS[name])
+            e.enable_opponent(o.pop("kind"), o.pop("lines"), seeds=[opponent_seed(s) for s in range(B)], **o)
+        envs[mode] = e
+    gens = {m: torch.Generator(device=dev) for m in envs}
+    for g in gens.values():
+        g.manual_seed(0)
+    attacks = {m: 0 for m in envs}
+
+    def one(mode, count=False):
+        e = envs[mode]
+        _, done, info = e.step_tensors(*draw(e, gens[mode], dev))
+        e.observe()
+        e.reset_instances(done.clone())
+        if count and "opponent_attack_line" in info:
+            attacks[mode] += int((info["opponent_attack_line"] >= 0).sum())
+
+    def timed(mode):
+        for _ in range(warmup):
+            one(mode)
+        torch.cuda.synchronize()
+        s0, o0 = envs[mode].engine.env_stats(), envs[mode].engine.obs_stats()
+        t0 = time.perf_counter()
+        for _ in range(steps):
+            one(mode)
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+        s1, o1 = envs[mode].engine.env_stats(), envs[mode].engine.obs_stats()
+        moved = (s1["h2d_bytes"] - s0["h2d_bytes"]) + (s1["d2h_bytes"] - s0["d2h_bytes"]) + (o1["d2h_bytes"] - o0["d2h_bytes"])
+        return B * steps / dt, moved / steps
+
+    res = {m: [] for m in envs}
+    for _ in range(repeats):
+        for m in ("off", "on"):
+            res[m].append(timed(m))
+    one("on", count=True)
+    for m in ("off", "on"):
+        r = np.array([x[0] for x in res[m]])
+        print(f"{name:28s} B={B:5d} prot={int(protections)} opponent {m:3s}: env.step/s min {r.min():.3e} median {np.median(r):.3e} "
+              f"max {r.max():.3e}; bytes moved per step {np.median([x[1] for x in res[m]]) / 1e3:.1f} kB")
+    print(f"{'':28s} attacks running in the last step: {attacks['on']} of {B}")
+    for e in envs.values():
+        e.close()
+
+
+def main():
+    from bench_env_tensor import card
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--repeats", type=int, default=5)
+    args = ap.parse_args()
+    print("card, power limit:", card())
+    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024)):
+        for prot in (False, True):
+            run(name, B, prot, args.steps, args.warmup, args.repeats)
+
+
+if __name__ == "__main__":
+    main()
