@@ -53,7 +53,7 @@ template <int T, int G, bool UNI> __device__ __forceinline__ int pb_any(unsigned
 // Lane 0 of every warp adds the SM cycles (clock64) spent between consecutive phase boundaries of solve_block to
 // pb_phase_clk[phase] (summed over the Newton iterations, the warps and the launches until the host reads and clears it);
 // pf_kernel_block adds every warp's cycle and globaltimer spans, from which the host converts cycles to time.
-enum { PC_STAGE, PC_ROW, PC_SUMS, PC_DCINV, PC_DCANG, PC_LINES, PC_BUSES, PC_STREAM, PC_UPDATE, PC_OUT, PC_N_PHASE,
+enum { PC_STAGE, PC_ROW, PC_SUMS, PC_DCINV, PC_DCANG, PC_BUSES, PC_STREAM, PC_UPDATE, PC_OUT, PC_N_PHASE,
        PC_SOLVES = PC_N_PHASE, PC_WARPS, PC_CYCLES, PC_NS, PC_SLOTS };
 __device__ unsigned long long pb_phase_clk[PC_SLOTS];
 #define PB_CLOCK_ON 1
@@ -263,77 +263,50 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         if (bad) PB_FAIL(ST_DIV, 0)
     }
     // ---- 3. Newton-Raphson ---------------------------------------------------------------------------------
-    // Four phases per iteration: [lane = line: branch currents + off-diagonal blocks] [lane = bus: S(V), mismatch, diagonal
-    // block + right-hand side; vote] [block operation stream] [lane = bus: state update; clear the off-diagonal blocks].
+    // Three phases per iteration: [lane = bus: I = Y V from the plan's admittance row, S(V), mismatch, the bus's whole block
+    // row + right-hand side; vote] [block operation stream] [lane = bus: state update; clear the fill-in blocks].
     int iters = 0;
     if (!is_dc) {
-        const uint16_t *bdpos = U16(o_bdpos), *bjpos = U16(o_bjpos), *rnd = U16(o_round), *bzero = U16(o_bzero), *late = U16(o_late);
-        const double *ydiag = F64(o_ydiag);
+        const uint16_t *bdpos = U16(o_bdpos), *bzero = U16(o_bzero), *yptr = U16(o_yptr), *ynb = U16(o_ynb), *yblk = U16(o_yblk);
+        const double *ydiag = F64(o_ydiag), *yval = F64(o_yval);
         const uint2 *bops = reinterpret_cast<const uint2 *>(blob + H.o_bops);
-        const int n_brow = H.n_brow, n_round = H.n_round, n_bzero = H.n_bzero, n_late = H.n_late;
+        const int n_brow = H.n_brow, n_bzero = H.n_bzero;
         bool conv = false, running = fstat < 0;
         PF_PHASE { for (int k = tid; k < n_bzero; k += T) A4[IX(bzero[k])] = make_float4(0.f, 0.f, 0.f, 0.f); }
         PB_SYNC();
         PB_CLOCK(PC_DCANG)
-        // off-diagonal blocks of line l: block (f, t) += [ti tr; -tr ti] with T = Vf conj(yft Vt), rows of a PV bus f keep only
-        // the P row, columns of a PV bus t only the theta column; same for (t, f).  Two separate read-modify-writes (a line
-        // with both ends on one bus hits the same block twice).
-#define PB_OFFDIAG(l, Vf, Vt, y, f, t)                                                                             \
-        {                                                                                                          \
-            const float ef = (float)(Vf).x, ff = (float)(Vf).y, et = (float)(Vt).x, ft = (float)(Vt).y;            \
-            const bool pqf = p_colv[f] != 0xFFFF, pqt = p_colv[t] != 0xFFFF;                                       \
-            const int b0 = bjpos[2 * (l)], b1 = bjpos[2 * (l) + 1];                                                \
-            {                                                                                                      \
-                const float yr = (float)(y)[2], yi = (float)(y)[3];                                                \
-                const float ar = yr * et - yi * ft, ai = yr * ft + yi * et;                                        \
-                const float tr = ef * ar + ff * ai, ti = ff * ar - ef * ai;                                        \
-                float4 b = A4[IX(b0)];                                                                             \
-                b.x += ti; if (pqt) b.y += tr; if (pqf) { b.z -= tr; if (pqt) b.w += ti; }                         \
-                A4[IX(b0)] = b;                                                                                    \
-            }                                                                                                      \
-            {                                                                                                      \
-                const float yr = (float)(y)[4], yi = (float)(y)[5];                                                \
-                const float ar = yr * ef - yi * ff, ai = yr * ff + yi * ef;                                        \
-                const float tr = et * ar + ft * ai, ti = ft * ar - et * ai;                                        \
-                float4 b = A4[IX(b1)];                                                                             \
-                b.x += ti; if (pqf) b.y += tr; if (pqt) { b.z -= tr; if (pqf) b.w += ti; }                         \
-                A4[IX(b1)] = b;                                                                                    \
-            }                                                                                                      \
-        }
         for (int it = 0;; ++it) {
-            PF_PHASE {                                         // lane = line: currents at both ends, off-diagonal blocks (round 0)
-                PB_LOOP for (int l = tid; l < nl; l += T) {
-                    const int f = p_brf[l];
-                    if (f == 0xFFFF) continue;
-                    const int t = p_brt[l];
-                    const double2 Vf = V[IX(f)], Vt = V[IX(t)];
-                    const double *y = line_y + (size_t)l * 8;
-                    cur[IX(2 * l)] = make_double2(y[0] * Vf.x - y[1] * Vf.y + y[2] * Vt.x - y[3] * Vt.y,
-                                                  y[0] * Vf.y + y[1] * Vf.x + y[2] * Vt.y + y[3] * Vt.x);
-                    cur[IX(2 * l + 1)] = make_double2(y[4] * Vf.x - y[5] * Vf.y + y[6] * Vt.x - y[7] * Vt.y,
-                                                      y[4] * Vf.y + y[5] * Vf.x + y[6] * Vt.y + y[7] * Vt.x);
-                    if (n_round <= 1 || rnd[l] == 0) PB_OFFDIAG(l, Vf, Vt, y, f, t)
-                }
-            }
-            PB_SYNC();
-            PB_CLOCK(PC_LINES)
             int viol = 0, wild = 0;
-            PF_PHASE {                                         // lane = bus: S = V conj(I), mismatch, diagonal block, right-hand side
+            PF_PHASE {                                         // lane = bus: S = V conj(I), mismatch, block row, right-hand side
                 PB_LOOP for (int i = tid; i < nb; i += T) {
                     const double2 Vi = V[IX(i)];
-                    double ir = 0.0, ii = 0.0, gs = 0.0, bs = 0.0;
+                    double gs = ydiag[2 * i], bs = ydiag[2 * i + 1];           // Y_ii + shunt
                     const int sx = shidx[i];
-                    if (sx != 0xFFFF) { gs = gsh[IX(sx)]; bs = bsh[IX(sx)]; ir = gs * Vi.x - bs * Vi.y; ii = gs * Vi.y + bs * Vi.x; }
-                    for (int e = adj_ptr[i]; e < adj_ptr[i + 1]; ++e) { const double2 c2 = cur[IX(adj[e])]; ir += c2.x; ii += c2.y; }
+                    if (sx != 0xFFFF) { gs += gsh[IX(sx)]; bs += bsh[IX(sx)]; }
+                    double ir = gs * Vi.x - bs * Vi.y, ii = gs * Vi.y + bs * Vi.x;
+                    // off-diagonal block (i, j) = [ti tr; -tr ti] with T = Vi conj(Y_ij Vj) (fp32), the Q row of a PV bus i and
+                    // the |V| column of a PV bus j zero; written whole (the reference bus's row goes to the dummy block)
+                    const bool pq = p_colv[i] != 0xFFFF;
+                    const float ei = (float)Vi.x, fi = (float)Vi.y;
+                    for (int e = yptr[i]; e < yptr[i + 1]; ++e) {
+                        const int j = ynb[e];
+                        const double2 Vj = V[IX(j)];
+                        const double yr = yval[2 * e], yi = yval[2 * e + 1];
+                        ir += yr * Vj.x - yi * Vj.y; ii += yr * Vj.y + yi * Vj.x;
+                        const float ej = (float)Vj.x, fj = (float)Vj.y, yrf = (float)yr, yif = (float)yi;
+                        const float ar = yrf * ej - yif * fj, ai = yrf * fj + yif * ej;
+                        const float tr = ei * ar + fi * ai, ti = fi * ar - ei * ai;
+                        const bool pqj = p_colv[j] != 0xFFFF;
+                        A4[IX(yblk[e])] = make_float4(ti, pqj ? tr : 0.f, pq ? -tr : 0.f, (pq && pqj) ? ti : 0.f);
+                    }
                     const double P = Vi.x * ir + Vi.y * ii, Q = Vi.y * ir - Vi.x * ii;
                     Pc[IX(i)] = P; Qc[IX(i)] = Q;
                     const int bd = bdpos[i];                                  // (0xFFFF: reference bus)
                     if (bd == 0xFFFF) continue;
-                    const bool pq = p_colv[i] != 0xFFFF;
                     const double dP = psp[IX(i)] - P;
                     { const double m1 = fabs(dP); viol |= !(m1 < a.tol_pu); wild |= !(m1 < 1e200); }
                     const float vi2 = (float)(Vi.x * Vi.x + Vi.y * Vi.y), Pf = (float)P, Qf = (float)Q;
-                    const float gi_ = (float)(ydiag[2 * i] + gs), bi_ = (float)(ydiag[2 * i + 1] + bs);
+                    const float gi_ = (float)gs, bi_ = (float)bs;
                     float4 D = make_float4(-Qf - bi_ * vi2, 0.f, 0.f, 1.f), R = make_float4((float)dP, 0.f, 0.f, 0.f);
                     if (pq) {
                         const double dQ = qsp[IX(i)] - Q;
@@ -363,19 +336,6 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 if (!viol) { conv = true; iters = it; break; }
                 wild = PB_ANY(wild);
                 if (it >= a.max_iter || wild) { iters = it; break; }
-            }
-            for (int r = 1, q = 0; r < n_round; ++r) {         // parallel lines / lines inside one bus: later rounds, one barrier each (rare)
-                PF_PHASE {
-                    for (int k = q + tid; k < n_late && late[2 * k + 1] == r; k += T) {
-                        const int l = late[2 * k];
-                        const int f = p_brf[l], t = p_brt[l];
-                        const double2 Vf = V[IX(f)], Vt = V[IX(t)];
-                        const double *y = line_y + (size_t)l * 8;
-                        PB_OFFDIAG(l, Vf, Vt, y, f, t)
-                    }
-                }
-                while (q < n_late && late[2 * q + 1] == r) ++q;
-                PB_SYNC();
             }
             // block LU + triangular solves: the plan's operation stream.  A row = T * U slots, lane j executes slots
             // j, j + T, ..., all loads of its U operations before any store; rows prefetched one ahead.
@@ -472,13 +432,12 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                         V[IX(i)] = make_double2(vmi * c2, vmi * s);
                     }
                 }
-                // (the bus lanes above read right-hand-side blocks only; the cleared set holds off-diagonal blocks)
+                // (the bus lanes above read right-hand-side blocks only; the cleared set holds the fill-in blocks)
                 PB_LOOP for (int k = tid; k < n_bzero; k += T) A4[IX(bzero[k])] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
             PB_SYNC();
             PB_CLOCK(PC_UPDATE)
         }
-#undef PB_OFFDIAG
         if (!conv) PB_FAIL(ST_DIV, iters)
     } else {
         // DC: line lanes compute flows from the angles, bus lanes sum them for the slack share
@@ -531,7 +490,13 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                     double pf, qf, pt, qt, sf, st;
                     if (is_dc) { pf = cur[IX(2 * l)].x * base; pt = -pf; qf = 0.0; qt = 0.0; sf = fabs(pf); st = sf; }
                     else {
-                        const double2 Aa = V[IX(f)], Bb = V[IX(t)], If = cur[IX(2 * l)], It = cur[IX(2 * l + 1)];
+                        // branch currents at both ends from the converged V (the Newton loop works on bus currents only)
+                        const double2 Aa = V[IX(f)], Bb = V[IX(t)];
+                        const double *y = line_y + (size_t)l * 8;
+                        const double2 If = make_double2(y[0] * Aa.x - y[1] * Aa.y + y[2] * Bb.x - y[3] * Bb.y,
+                                                        y[0] * Aa.y + y[1] * Aa.x + y[2] * Bb.y + y[3] * Bb.x);
+                        const double2 It = make_double2(y[4] * Aa.x - y[5] * Aa.y + y[6] * Bb.x - y[7] * Bb.y,
+                                                        y[4] * Aa.y + y[5] * Aa.x + y[6] * Bb.y + y[7] * Bb.x);
                         pf = (Aa.x * If.x + Aa.y * If.y) * base; qf = (Aa.y * If.x - Aa.x * If.y) * base;
                         pt = (Bb.x * It.x + Bb.y * It.y) * base; qt = (Bb.y * It.x - Bb.x * It.y) * base;
                         sf = sqrt(pf * pf + qf * qf); st = sqrt(pt * pt + qt * qt);

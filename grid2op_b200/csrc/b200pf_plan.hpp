@@ -64,6 +64,8 @@ struct PlanHeader {
     int total_bytes;
     // per bus (nb entries each)
     int o_slot, o_btype, o_colth, o_colv, o_dcidx, o_vmunit, o_cnt, o_nref, o_dpos /* [nb][4] */;
+    // ydiag: sum of y_ff / y_tt over the bus's line ends; block plans: the full Y_ii (a line with both ends on the bus adds
+    // y_ft + y_tf too)
     int o_qmins, o_qmaxs, o_ydiag /* [nb][2] */, o_dcshift;                               // doubles
     int o_adj_ptr, o_adj, o_bu_ptr, o_bu, o_bl_ptr, o_bl, o_bs_ptr, o_bs, o_bh_ptr, o_bh;  // CSR lists (u16)
     // per line
@@ -89,9 +91,16 @@ struct PlanHeader {
     int o_bops;            // 8-byte slots {u16 d, a, b, flags}: BYTE offsets (16 * blk_G * block index) into the value array;
                            // flags bit 0: barrier after this row, bit 1: row type (0: D -= A B, 1: D = inv(A) D)
     int o_bdpos;           // u16 [nb]: block index of the diagonal block of the bus (0xFFFF: reference bus)
-    int o_bjpos;           // u16 [n_line][2]: block (from,to) and (to,from) of the line (dummy when an end is a reference bus)
-    int o_bzero, n_bzero;  // u16 block indices cleared before every assembly (all off-diagonal blocks incl. fill)
+    int o_bjpos;           // u16 [n_line][2]: block (from,to) and (to,from) of the line (dummy when an end is a reference bus;
+                           // validation: the kernel assembles from the admittance rows)
+    int o_bzero, n_bzero;  // u16 block indices cleared before every assembly (the pure fill-in blocks)
     int o_bpass_ptr;       // int32 [n_bpass + 1] slot range of every pass (validation)
+    // admittance rows of the buses, CSR, neighbours in ascending bus order: Y_ij summed over the lines between i and j in line
+    // order (y_ft at a from end, y_tf at a to end), and the off-diagonal block (dcidx i, dcidx j) the lane of bus i writes
+    // (dummy when either end is a reference bus)
+    int o_yptr, o_ynb;     // u16 [nb + 1] row pointer, u16 neighbour bus per entry
+    int o_yval;            // fp64 [entries][2]: Y_ij
+    int o_yblk;            // u16 per entry: block index
     int pad2[1];
 };
 static_assert(sizeof(PlanHeader) % 16 == 0, "plan blobs are concatenated 16-byte aligned");
@@ -279,7 +288,8 @@ public:
         std::vector<uint16_t> dpos, jpos, zero;
         int nblk = 0, nblkA = 0, n_brow = 0, n_bpass = 0;            // block plans
         std::vector<BOp> bops;
-        std::vector<int> bdpos(nb, -1), bjpos((size_t)nl * 2, -1), bzero, bpass_ptr(1, 0);
+        std::vector<int> bdpos(nb, -1), bjpos((size_t)nl * 2, -1), bzero, bpass_ptr(1, 0), yptr, ynb, yblk;
+        std::vector<double> yval;
         if (!blk_) {
         // ---- scalar pattern of the Jacobian, symbolic LU --------------------------------------------
         std::vector<char> S((size_t)d * d, 0);
@@ -543,31 +553,44 @@ public:
             for (int q = 0; q < W; ++q) emit(BD, BD, BD, 0);          // guard row: the prefetch of "the row after the last" reads it
             // ---- assembly positions ------------------------------------------------------------------------
             for (int i = 0; i < nb; ++i) if (dcidx[i] >= 0) bdpos[i] = BP(dcidx[i], dcidx[i]);
+            for (int l = 0; l < nl; ++l) {
+                const int f = brf[l], t = brt[l];
+                bjpos[(size_t)2 * l] = BD; bjpos[(size_t)2 * l + 1] = BD;
+                if (f < 0) continue;
+                const int cf = dcidx[f], ct = dcidx[t];
+                if (cf >= 0 && ct >= 0) { bjpos[(size_t)2 * l] = BP(cf, ct); bjpos[(size_t)2 * l + 1] = BP(ct, cf); }
+            }
+            // ---- admittance rows: the bus lane of bus i computes its current from them and writes the off-diagonal blocks of
+            //      its block row whole, so every block of the bus graph has exactly one writer per Newton evaluation (parallel
+            //      lines are summed here; a line with both ends on one bus is part of Y_ii, below) and only the fill is cleared
             {
-                std::vector<std::vector<char>> used;
+                std::vector<std::vector<std::pair<int, int>>> ends(nb);          // (neighbour bus, 2 * line + side)
                 for (int l = 0; l < nl; ++l) {
                     const int f = brf[l], t = brt[l];
-                    bjpos[(size_t)2 * l] = BD; bjpos[(size_t)2 * l + 1] = BD;
-                    if (f < 0) continue;
-                    const int cf = dcidx[f], ct = dcidx[t];
-                    if (cf >= 0 && ct >= 0) { bjpos[(size_t)2 * l] = BP(cf, ct); bjpos[(size_t)2 * l + 1] = BP(ct, cf); }
-                    // round 0 is added BEFORE the bus lanes assign the diagonal blocks: a line with both ends on one bus (it
-                    // adds into a diagonal block) must come later
-                    int r = (f == t) ? 1 : 0;
-                    for (;; ++r) {
-                        while (r >= (int)used.size()) used.emplace_back(nblkA + 1, 0);
-                        bool clash = false;
-                        for (int q = 0; q < 2; ++q) { const int p = bjpos[(size_t)2 * l + q]; if (p != BD && used[r][p]) clash = true; }
-                        if (!clash) break;
-                    }
-                    for (int q = 0; q < 2; ++q) { const int p = bjpos[(size_t)2 * l + q]; if (p != BD) used[r][p] = 1; }
-                    round[l] = r; n_round = std::max(n_round, r + 1);
+                    if (f < 0 || f == t) continue;
+                    ends[f].push_back({t, 2 * l}); ends[t].push_back({f, 2 * l + 1});
                 }
-            }
-            {
-                std::vector<char> isdiag(nblk, 0);
-                for (int k = 0; k < n1; ++k) isdiag[BP(k, k)] = 1;
-                for (int p = 0; p < nblk; ++p) if (!isdiag[p]) bzero.push_back(p);
+                std::vector<char> written(nblk, 0);
+                yptr.assign(1, 0);
+                for (int i = 0; i < nb; ++i) {
+                    std::sort(ends[i].begin(), ends[i].end());                   // neighbours ascending, then line order
+                    for (size_t e = 0; e < ends[i].size();) {
+                        const int j = ends[i][e].first;
+                        double yr = 0.0, yi = 0.0;
+                        for (; e < ends[i].size() && ends[i][e].first == j; ++e) {
+                            const int l = ends[i][e].second >> 1, side = ends[i][e].second & 1;
+                            const double *y = &g.line_y[(size_t)l * 8 + (side ? 4 : 2)];     // y_ft at the from end, y_tf at the to end
+                            yr += y[0]; yi += y[1];
+                        }
+                        const int ci = dcidx[i], cj = dcidx[j];
+                        const int b = (ci >= 0 && cj >= 0) ? BP(ci, cj) : BD;
+                        if (b != BD) written[b] = 1;
+                        ynb.push_back(j); yval.push_back(yr); yval.push_back(yi); yblk.push_back(b);
+                    }
+                    yptr.push_back((int)ynb.size());
+                }
+                for (int k = 0; k < n1; ++k) written[BP(k, k)] = 1;
+                for (int p = 0; p < nblk; ++p) if (!written[p]) bzero.push_back(p);
             }
         }
         // ---- static per-bus line data ------------------------------------------------------------------
@@ -579,6 +602,7 @@ public:
             const double *y = &g.line_y[(size_t)l * 8];
             ydiag[(size_t)f * 2] += y[0]; ydiag[(size_t)f * 2 + 1] += y[1];
             ydiag[(size_t)t * 2] += y[6]; ydiag[(size_t)t * 2 + 1] += y[7];
+            if (blk_ && f == t) { ydiag[(size_t)f * 2] += y[2] + y[4]; ydiag[(size_t)f * 2 + 1] += y[3] + y[5]; }
             dcshift[f] += g.line_pshift[l]; dcshift[t] -= g.line_pshift[l];
             adj[f].push_back(2 * l); adj[t].push_back(2 * l + 1);
         }
@@ -794,7 +818,8 @@ public:
         H.o_dpos = put_u16v(dpos);
         put_csr(adj, H.o_adj_ptr, H.o_adj); put_csr(bu, H.o_bu_ptr, H.o_bu); put_csr(bl, H.o_bl_ptr, H.o_bl);
         put_csr(bs, H.o_bs_ptr, H.o_bs); put_csr(bh, H.o_bh_ptr, H.o_bh);
-        H.o_brf = put_u16(brf); H.o_brt = put_u16(brt); H.o_round = put_u16(round); H.o_jpos = put_u16v(jpos);
+        H.o_brf = put_u16(brf); H.o_brt = put_u16(brt);
+        if (!blk_) { H.o_round = put_u16(round); H.o_jpos = put_u16v(jpos); }
         H.o_unit_bus = put_u16(unit_bus); H.o_load_bus = put_u16(load_bus); H.o_sto_bus = put_u16(sto_bus); H.o_sh_bus = put_u16(sh_bus);
         {
             std::vector<int> shidx(nb, -1);
@@ -802,18 +827,20 @@ public:
             for (int i = 0; i < nb; ++i) if (!bh[i].empty()) shidx[i] = n_shb++;
             H.o_shidx = put_u16(shidx); H.n_shb = n_shb;
         }
-        {
+        if (!blk_) {
             std::vector<int> late;
             for (int r = 1; r < n_round; ++r) for (int l = 0; l < nl; ++l) if (brf[l] >= 0 && round[l] == r) { late.push_back(l); late.push_back(r); }
             H.o_late = put_u16(late); H.n_late = (int)late.size() / 2;
+            H.o_zero = put_u16v(zero);
         }
-        H.o_zero = put_u16v(zero);
         if (blk_) {
             align(8);
             H.o_bops = (int)blob.size();
             blob.resize(blob.size() + bops.size() * sizeof(BOp));
             if (!bops.empty()) memcpy(&blob[H.o_bops], bops.data(), bops.size() * sizeof(BOp));
+            H.o_yval = put_d(yval);
             H.o_bdpos = put_u16(bdpos); H.o_bjpos = put_u16(bjpos); H.o_bzero = put_u16(bzero); H.o_bpass_ptr = put_i32(bpass_ptr);
+            H.o_yptr = put_u16(yptr); H.o_ynb = put_u16(ynb); H.o_yblk = put_u16(yblk);
         }
         PLAN_TICK("serialise");
         align(16);

@@ -10,7 +10,7 @@ the same warps measured (their globaltimer span over their clock64 span).  Print
 
     python scripts/phase_clock.py [--out DIR] [--lib PREBUILT.so] [--steps 200] [--warmup 10] [--batch 4096]
 
-The instrumented kernel reads the clock 3 + 4 x iterations times per warp, so its phases add up to a little more than the
+The instrumented kernel reads the clock 3 + 3 x iterations times per warp, so its phases add up to a little more than the
 production kernel's step; use the table for where the time goes, bench.py for how long a step takes."""
 import argparse
 import ctypes
@@ -27,17 +27,17 @@ sys.path.insert(0, REPO)
 GOLD = os.path.join(REPO, "tests", "golden")
 
 # counters of b200pf_block.cuh (PC_*), in order
-PHASES = ["stage", "row", "sums", "dc_inverse", "dc_angles", "nr_lines", "nr_buses_vote", "nr_stream", "nr_update", "outputs"]
+PHASES = ["stage", "row", "sums", "dc_inverse", "dc_angles", "nr_buses_vote", "nr_stream", "nr_update", "outputs"]
 WHAT = {"stage": "kernel entry -> plan + static arrays staged (staged launches: the first rows are loaded meanwhile)",
         "row": "chronics row into the workspace (when not loaded during the staging)",
         "sums": "phase 1: per-bus sums of the injections, DC right-hand side",
         "dc_inverse": "DC angles = plan inverse x right-hand side",
-        "dc_angles": "angles into the workspace, sincos, clearing of the off-diagonal blocks",
-        "nr_lines": "Newton, all iterations: branch currents + off-diagonal blocks (lane = line)",
-        "nr_buses_vote": "Newton, all iterations: S(V), mismatch, diagonal blocks, convergence vote (lane = bus)",
+        "dc_angles": "angles into the workspace, sincos, clearing of the fill-in blocks",
+        "nr_buses_vote": "Newton, all iterations: I = Y V from the admittance rows, S(V), mismatch, the bus's block row "
+                         "(diagonal + off-diagonal blocks), convergence vote (lane = bus)",
         "nr_stream": "Newton, all iterations: block LU + solves (the plan's operation stream)",
-        "nr_update": "Newton, all iterations: state update, block clearing (lane = bus)",
-        "outputs": "loop exit -> result records, rho stored"}
+        "nr_update": "Newton, all iterations: state update, clearing of the fill-in blocks (lane = bus)",
+        "outputs": "loop exit -> branch currents, result records, rho stored"}
 N_SLOTS = len(PHASES) + 4          # + solves, warps, cycles, ns
 
 
