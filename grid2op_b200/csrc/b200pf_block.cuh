@@ -25,6 +25,8 @@
 namespace b200pf {
 
 #ifdef B200PF_EMULATE
+struct float2 { float x, y; };
+static inline float2 make_float2(float x, float y) { float2 r; r.x = x; r.y = y; return r; }
 #define PB_SYNC() ((void)0)
 #define PB_ANY(x) (x)
 #define PB_LOOP
@@ -119,11 +121,54 @@ PF_DEV void block_row_copy(const float *grow, int n, float *srow, int gi, int ti
 }
 
 // Byte offset of srow in a warp's workspace (the layout solve_block builds from the strides Lnb / LnblkA): value blocks, six
-// bus arrays, the shunt pair, V, the branch currents, then the row.
+// bus arrays, the shunt pair, V, the branch currents, V in fp32, then the row.
 template <int G>
 PF_DEV size_t block_srow_off(int Lnb, int LnblkA, int nsh, int nl) {
     const size_t Lb = (size_t)Lnb * G, LA = (size_t)(LnblkA + 1) * G;
-    return LA * 16 + (6 * Lb + 2 * (size_t)nsh * G) * 8 + (Lb + 2 * (size_t)nl * G) * 16;
+    return LA * 16 + (6 * Lb + 2 * (size_t)nsh * G) * 8 + (Lb + 2 * (size_t)nl * G) * 16 + Lb * 8;
+}
+
+// A bus's diagonal block, right-hand side and mismatch tests from its S = P + jQ (fp64) in the Newton evaluation: a PV bus
+// keeps an identity Q row and no Q mismatch.  Arithmetic only, so that the two buses of a lane are independent chains.
+struct PbBusRow { float4 D, R; int viol, wild; };
+// (gi_, bi_: (float) of Y_ii + shunt)
+PF_DEV PbBusRow pb_bus_row(double2 Vi, double P, double Q, double ps, double qs, float gi_, float bi_, bool pq, double tol) {
+    PbBusRow r;
+    const double dP = ps - P;
+    { const double m1 = fabs(dP); r.viol = !(m1 < tol); r.wild = !(m1 < 1e200); }
+    const float vi2 = (float)(Vi.x * Vi.x + Vi.y * Vi.y), Pf = (float)P, Qf = (float)Q;
+    r.D = make_float4(-Qf - bi_ * vi2, 0.f, 0.f, 1.f); r.R = make_float4((float)dP, 0.f, 0.f, 0.f);
+    if (pq) {
+        const double dQ = qs - Q;
+        { const double m2 = fabs(dQ); r.viol |= !(m2 < tol); r.wild |= !(m2 < 1e200); }
+        r.D.y = Pf + gi_ * vi2; r.D.z = Pf - gi_ * vi2; r.D.w = Qf - bi_ * vi2;
+        r.R.z = (float)dQ;
+    }
+    return r;
+}
+
+// State update of a bus from its solved step (dth, dvr = d|V| / |V|): V rotated by dth with the Taylor series of sin / cos
+// (remainder < 3e-18 for |x| < 0.25) and scaled by 1 + dvr.  Arithmetic only; `small` false: the caller takes the sincos
+// path (pb_update_slow) instead.
+struct PbUpd { double2 V; double vm, va; bool small; };
+PF_DEV PbUpd pb_update_small(double2 Vo, double vmi, double vai, double dth, double dvr) {
+    PbUpd r;
+    r.va = vai + dth;
+    r.vm = vmi * (1.0 + dvr);
+    r.small = fabs(dth) < 0.25 && r.vm > 0.0;
+    const double x2 = dth * dth;
+    const double sn = dth * (1.0 - x2 * (1.0 / 6.0) * (1.0 - x2 * (1.0 / 20.0) * (1.0 - x2 * (1.0 / 42.0) * (1.0 - x2 * (1.0 / 72.0) *
+                      (1.0 - x2 * (1.0 / 110.0) * (1.0 - x2 * (1.0 / 156.0)))))));
+    const double cs = 1.0 - x2 * 0.5 * (1.0 - x2 * (1.0 / 12.0) * (1.0 - x2 * (1.0 / 30.0) * (1.0 - x2 * (1.0 / 56.0) * (1.0 - x2 * (1.0 / 90.0) *
+                      (1.0 - x2 * (1.0 / 132.0) * (1.0 - x2 * (1.0 / 182.0)))))));
+    const double scl = 1.0 + dvr;
+    r.V = make_double2(scl * (Vo.x * cs - Vo.y * sn), scl * (Vo.x * sn + Vo.y * cs));
+    return r;
+}
+PF_DEV void pb_update_slow(PbUpd &r) {
+    if (r.vm < 0.0) { r.vm = -r.vm; r.va += 3.14159265358979323846; }
+    double s, c2; PF_SINCOS(r.va, &s, &c2);
+    r.V = make_double2(r.vm * c2, r.vm * s);
 }
 
 // sm: workspace of the WARP (G instances, interleaved); gi: instance slot of this lane in the warp; tid0: lane of the instance
@@ -166,7 +211,7 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
 #undef PB_STAT
     const float *th_lim_ = STAGE ? reinterpret_cast<const float *>(pa.stat + pa.so.th_lim) : a.th_lim;
     const double *line_y = line_y_;
-    const uint16_t *p_colth = U16(o_colth), *p_colv = U16(o_colv), *p_dcidx = U16(o_dcidx);
+    const uint16_t *p_colth = U16(o_colth), *p_dcidx = U16(o_dcidx);
     const uint16_t *p_brf = U16(o_brf), *p_brt = U16(o_brt);
     const uint16_t *adj_ptr = U16(o_adj_ptr), *adj = U16(o_adj), *shidx = U16(o_shidx);
     // ---- workspace of the warp: every array holds G interleaved copies -------------------------------------------------
@@ -177,7 +222,8 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
            *gsh = Qc + Lb, *bsh = gsh + (size_t)nsh * G;
     double2 *V = reinterpret_cast<double2 *>(bsh + (size_t)nsh * G);
     double2 *cur = V + Lb;
-    float *srow = reinterpret_cast<float *>(cur + (size_t)2 * nl * G);
+    float2 *Vf = reinterpret_cast<float2 *>(cur + (size_t)2 * nl * G);    // (float) of V, written with it
+    float *srow = reinterpret_cast<float *>(Vf + Lb);
     // ---- injections of this instance ----------------------------------------------------------------------
     const bool has_row = MODE == 1 ? true : (a.series != 0);
     const bool is_dc = MODE == 1 ? false : (a.is_dc != 0);
@@ -256,7 +302,11 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
                 bad |= !(fabs(th) < 1e300);
                 const double vmi = vm[IX(i)];
                 if (is_dc) V[IX(i)] = make_double2(th, vmi);
-                else { double s, c2; PF_SINCOS(th, &s, &c2); V[IX(i)] = make_double2(vmi * c2, vmi * s); }
+                else {
+                    double s, c2; PF_SINCOS(th, &s, &c2);
+                    const double2 v = make_double2(vmi * c2, vmi * s);
+                    V[IX(i)] = v; Vf[IX(i)] = make_float2((float)v.x, (float)v.y);
+                }
             }
         }
         bad = PB_ANY(bad);
@@ -267,8 +317,11 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
     // row + right-hand side; vote] [block operation stream] [lane = bus: state update; clear the fill-in blocks].
     int iters = 0;
     if (!is_dc) {
-        const uint16_t *bdpos = U16(o_bdpos), *bzero = U16(o_bzero), *yptr = U16(o_yptr), *ynb = U16(o_ynb), *yblk = U16(o_yblk);
+        const uint16_t *bzero = U16(o_bzero), *yptr = U16(o_yptr);
         const double *ydiag = F64(o_ydiag), *yval = F64(o_yval);
+        const unsigned *yword = reinterpret_cast<const unsigned *>(blob + H.o_yword);
+        const float2 *yf32 = reinterpret_cast<const float2 *>(blob + H.o_yf32);
+        const uint2 *bdesc = reinterpret_cast<const uint2 *>(blob + H.o_bdesc);
         const uint2 *bops = reinterpret_cast<const uint2 *>(blob + H.o_bops);
         const int n_brow = H.n_brow, n_bzero = H.n_bzero;
         bool conv = false, running = fstat < 0;
@@ -278,44 +331,71 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
         for (int it = 0;; ++it) {
             int viol = 0, wild = 0;
             PF_PHASE {                                         // lane = bus: S = V conj(I), mismatch, block row, right-hand side
-                PB_LOOP for (int i = tid; i < nb; i += T) {
-                    const double2 Vi = V[IX(i)];
-                    double gs = ydiag[2 * i], bs = ydiag[2 * i + 1];           // Y_ii + shunt
-                    const int sx = shidx[i];
-                    if (sx != 0xFFFF) { gs += gsh[IX(sx)]; bs += bsh[IX(sx)]; }
-                    double ir = gs * Vi.x - bs * Vi.y, ii = gs * Vi.y + bs * Vi.x;
+                // A lane evaluates its buses i and i + T together, as two independent chains: the loads of both, then the
+                // arithmetic of both, then the stores of both (the compiler cannot move a load above a shared-memory store).
+                // Each bus keeps its own accumulators and summation order: (Y_ii + shunt) V_i, then its neighbours ascending.
+                PB_LOOP for (int i = tid; i < nb; i += 2 * T) {
+                    const int i2 = i + T < nb ? i + T : i;    // (no second bus: chain 2 re-reads bus i and stores nothing)
+                    const bool two = i2 != i;
+                    const uint2 da = bdesc[i], db = bdesc[i2];
+                    const float2 Fa = Vf[IX(i)], Fb = Vf[IX(i2)];
+                    double gsa = ydiag[2 * i], bsa = ydiag[2 * i + 1], gsb = ydiag[2 * i2], bsb = ydiag[2 * i2 + 1];   // Y_ii + shunt
+                    const int ea = yptr[i], na = yptr[i + 1] - ea, eb = yptr[i2], nbb = two ? yptr[i2 + 1] - eb : 0;
+                    unsigned wa = yword[na > 0 ? ea : 0], wb = yword[nbb > 0 ? eb : 0];      // (the plan stores at least one entry)
+                    const int sxa = da.y & 0xFFFF, sxb = db.y & 0xFFFF;
+                    if (sxa != 0xFFFF) { gsa += gsh[IX(sxa)]; bsa += bsh[IX(sxa)]; }
+                    if (sxb != 0xFFFF) { gsb += gsh[IX(sxb)]; bsb += bsh[IX(sxb)]; }
+                    double ira, iia, irb, iib;
+                    {
+                        const double2 Va = V[IX(i)], Vb = V[IX(i2)];
+                        ira = gsa * Va.x - bsa * Va.y; iia = gsa * Va.y + bsa * Va.x;
+                        irb = gsb * Vb.x - bsb * Vb.y; iib = gsb * Vb.y + bsb * Vb.x;
+                    }
+                    const float gfa = (float)gsa, bfa = (float)bsa, gfb = (float)gsb, bfb = (float)bsb;
                     // off-diagonal block (i, j) = [ti tr; -tr ti] with T = Vi conj(Y_ij Vj) (fp32), the Q row of a PV bus i and
-                    // the |V| column of a PV bus j zero; written whole (the reference bus's row goes to the dummy block)
-                    const bool pq = p_colv[i] != 0xFFFF;
-                    const float ei = (float)Vi.x, fi = (float)Vi.y;
-                    for (int e = yptr[i]; e < yptr[i + 1]; ++e) {
-                        const int j = ynb[e];
-                        const double2 Vj = V[IX(j)];
-                        const double yr = yval[2 * e], yi = yval[2 * e + 1];
-                        ir += yr * Vj.x - yi * Vj.y; ii += yr * Vj.y + yi * Vj.x;
-                        const float ej = (float)Vj.x, fj = (float)Vj.y, yrf = (float)yr, yif = (float)yi;
-                        const float ar = yrf * ej - yif * fj, ai = yrf * fj + yif * ej;
-                        const float tr = ei * ar + fi * ai, ti = fi * ar - ei * ai;
-                        const bool pqj = p_colv[j] != 0xFFFF;
-                        A4[IX(yblk[e])] = make_float4(ti, pqj ? tr : 0.f, pq ? -tr : 0.f, (pq && pqj) ? ti : 0.f);
+                    // the |V| column of a PV bus j zero; written whole (the reference bus's row goes to the dummy block).  Entry k
+                    // of both rows per round; the entry words of the next round are loaded before this round's stores.
+                    const bool pqa = (da.y >> 16) != 0u, pqb = (db.y >> 16) != 0u;
+                    // (at least one round, so that no branch separates the loads above from their use: two empty rows add
+                    // nothing and store to the dummy block)
+                    const int nk = na > nbb ? na : nbb;
+                    int k = 0;
+                    PB_LOOP do {
+                        const bool ka = k < na, kb = k < nbb;
+                        const int qa = ka ? ea + k : 0, qb = kb ? eb + k : 0;
+                        const int ja = (wa >> 16) & 0x7FFF, jb = (wb >> 16) & 0x7FFF;
+                        const double2 Vja = V[IX(ja)], Vjb = V[IX(jb)];
+                        const float2 Fja = Vf[IX(ja)], Fjb = Vf[IX(jb)];
+                        const double yra = yval[2 * qa], yia = yval[2 * qa + 1], yrb = yval[2 * qb], yib = yval[2 * qb + 1];
+                        const float2 Ya = yf32[qa], Yb = yf32[qb];
+                        const unsigned wna = yword[k + 1 < na ? ea + k + 1 : 0], wnb = yword[k + 1 < nbb ? eb + k + 1 : 0];
+                        // (computed unconditionally, so that the compiler keeps every load of the round above its arithmetic;
+                        // a chain past its row adds nothing and stores to the dummy block)
+                        const double dra = yra * Vja.x - yia * Vja.y, dia = yra * Vja.y + yia * Vja.x;
+                        const double drb = yrb * Vjb.x - yib * Vjb.y, dib = yrb * Vjb.y + yib * Vjb.x;
+                        if (ka) { ira += dra; iia += dia; }
+                        if (kb) { irb += drb; iib += dib; }
+                        const float ara = Ya.x * Fja.x - Ya.y * Fja.y, aia = Ya.x * Fja.y + Ya.y * Fja.x;
+                        const float arb = Yb.x * Fjb.x - Yb.y * Fjb.y, aib = Yb.x * Fjb.y + Yb.y * Fjb.x;
+                        const float tra = Fa.x * ara + Fa.y * aia, tia = Fa.y * ara - Fa.x * aia;
+                        const float trb = Fb.x * arb + Fb.y * aib, tib = Fb.y * arb - Fb.x * aib;
+                        const bool pqja = (wa >> 31) != 0u, pqjb = (wb >> 31) != 0u;
+                        A4[IX(ka ? (int)(wa & 0xFFFF) : nblkA)] = make_float4(tia, pqja ? tra : 0.f, pqa ? -tra : 0.f, (pqa && pqja) ? tia : 0.f);
+                        A4[IX(kb ? (int)(wb & 0xFFFF) : nblkA)] = make_float4(tib, pqjb ? trb : 0.f, pqb ? -trb : 0.f, (pqb && pqjb) ? tib : 0.f);
+                        wa = wna; wb = wnb;
+                    } while (++k < nk);
+                    const double2 Va = V[IX(i)], Vb = V[IX(i2)];            // (read again: fewer registers live through the rows)
+                    const double Pa = Va.x * ira + Va.y * iia, Qa = Va.y * ira - Va.x * iia;
+                    const double Pb = Vb.x * irb + Vb.y * iib, Qb = Vb.y * irb - Vb.x * iib;
+                    const PbBusRow ra = pb_bus_row(Va, Pa, Qa, psp[IX(i)], qsp[IX(i)], gfa, bfa, pqa, a.tol_pu);
+                    const PbBusRow rb = pb_bus_row(Vb, Pb, Qb, psp[IX(i2)], qsp[IX(i2)], gfb, bfb, pqb, a.tol_pu);
+                    const int bda = da.x & 0xFFFF, bdb = db.x & 0xFFFF;            // (0xFFFF: reference bus)
+                    Pc[IX(i)] = Pa; Qc[IX(i)] = Qa;
+                    if (bda != 0xFFFF) { A4[IX(bda)] = ra.D; A4[IX(nblk + (da.x >> 16))] = ra.R; viol |= ra.viol; wild |= ra.wild; }
+                    if (two) {
+                        Pc[IX(i2)] = Pb; Qc[IX(i2)] = Qb;
+                        if (bdb != 0xFFFF) { A4[IX(bdb)] = rb.D; A4[IX(nblk + (db.x >> 16))] = rb.R; viol |= rb.viol; wild |= rb.wild; }
                     }
-                    const double P = Vi.x * ir + Vi.y * ii, Q = Vi.y * ir - Vi.x * ii;
-                    Pc[IX(i)] = P; Qc[IX(i)] = Q;
-                    const int bd = bdpos[i];                                  // (0xFFFF: reference bus)
-                    if (bd == 0xFFFF) continue;
-                    const double dP = psp[IX(i)] - P;
-                    { const double m1 = fabs(dP); viol |= !(m1 < a.tol_pu); wild |= !(m1 < 1e200); }
-                    const float vi2 = (float)(Vi.x * Vi.x + Vi.y * Vi.y), Pf = (float)P, Qf = (float)Q;
-                    const float gi_ = (float)gs, bi_ = (float)bs;
-                    float4 D = make_float4(-Qf - bi_ * vi2, 0.f, 0.f, 1.f), R = make_float4((float)dP, 0.f, 0.f, 0.f);
-                    if (pq) {
-                        const double dQ = qsp[IX(i)] - Q;
-                        { const double m2 = fabs(dQ); viol |= !(m2 < a.tol_pu); wild |= !(m2 < 1e200); }
-                        D.y = Pf + gi_ * vi2; D.z = Pf - gi_ * vi2; D.w = Qf - bi_ * vi2;
-                        R.z = (float)dQ;
-                    }
-                    A4[IX(bd)] = D;
-                    A4[IX(nblk + p_dcidx[i])] = R;
                 }
             }
             viol = PB_ANY(viol);
@@ -404,33 +484,22 @@ PF_DEV void solve_block(const DevGrid &g, const RunArgs &a, const PlanArgs &pa, 
             }
             PB_CLOCK(PC_STREAM)
             PF_PHASE {                                         // lane = bus: state update from the solved right-hand-side blocks
-                PB_LOOP for (int i = tid; i < ((!UNI || running) ? nb : 0); i += T) {
-                    const int c = p_dcidx[i];
-                    double vmi = vm[IX(i)], vai = va[IX(i)];
-                    float4 X = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (c != 0xFFFF) X = A4[IX(nblk + c)];
-                    const double dth = (double)X.x;
-                    const double dvr = (c != 0xFFFF && p_colv[i] != 0xFFFF) ? (double)X.z : 0.0;
-                    vai += dth;
-                    const double vnew = vmi * (1.0 + dvr);
-                    if (fabs(dth) < 0.25 && vnew > 0.0) {
-                        // small angle step: rotate (e, f) by dth with the Taylor series of sin / cos (remainder < 3e-18 for |x| < 0.25)
-                        const double x2 = dth * dth;
-                        const double sn = dth * (1.0 - x2 * (1.0 / 6.0) * (1.0 - x2 * (1.0 / 20.0) * (1.0 - x2 * (1.0 / 42.0) * (1.0 - x2 * (1.0 / 72.0) *
-                                          (1.0 - x2 * (1.0 / 110.0) * (1.0 - x2 * (1.0 / 156.0)))))));
-                        const double cs = 1.0 - x2 * 0.5 * (1.0 - x2 * (1.0 / 12.0) * (1.0 - x2 * (1.0 / 30.0) * (1.0 - x2 * (1.0 / 56.0) * (1.0 - x2 * (1.0 / 90.0) *
-                                          (1.0 - x2 * (1.0 / 132.0) * (1.0 - x2 * (1.0 / 182.0)))))));
-                        const double2 Vo = V[IX(i)];
-                        const double scl = 1.0 + dvr;
-                        V[IX(i)] = make_double2(scl * (Vo.x * cs - Vo.y * sn), scl * (Vo.x * sn + Vo.y * cs));
-                        vm[IX(i)] = vnew; va[IX(i)] = vai;
-                    } else {
-                        vmi = vnew;
-                        if (vmi < 0.0) { vmi = -vmi; vai += 3.14159265358979323846; }
-                        vm[IX(i)] = vmi; va[IX(i)] = vai;
-                        double s, c2; PF_SINCOS(vai, &s, &c2);
-                        V[IX(i)] = make_double2(vmi * c2, vmi * s);
-                    }
+                // buses i and i + T of a lane as two independent chains, like the evaluation above
+                PB_LOOP for (int i = tid; i < ((!UNI || running) ? nb : 0); i += 2 * T) {
+                    const int i2 = i + T < nb ? i + T : i;
+                    const uint2 da = bdesc[i], db = bdesc[i2];
+                    const int ca = da.x >> 16, cb = db.x >> 16;               // (0xFFFF: reference bus, no step)
+                    const float4 Xa = A4[IX(ca != 0xFFFF ? nblk + ca : nblkA)], Xb = A4[IX(cb != 0xFFFF ? nblk + cb : nblkA)];
+                    const double2 Voa = V[IX(i)], Vob = V[IX(i2)];
+                    const double vma = vm[IX(i)], vaa = va[IX(i)], vmb = vm[IX(i2)], vab = va[IX(i2)];
+                    const double dtha = ca != 0xFFFF ? (double)Xa.x : 0.0, dthb = cb != 0xFFFF ? (double)Xb.x : 0.0;
+                    const double dvra = (ca != 0xFFFF && (da.y >> 16) != 0u) ? (double)Xa.z : 0.0;
+                    const double dvrb = (cb != 0xFFFF && (db.y >> 16) != 0u) ? (double)Xb.z : 0.0;
+                    PbUpd ua = pb_update_small(Voa, vma, vaa, dtha, dvra), ub = pb_update_small(Vob, vmb, vab, dthb, dvrb);
+                    if (!ua.small) pb_update_slow(ua);
+                    if (!ub.small) pb_update_slow(ub);
+                    V[IX(i)] = ua.V; Vf[IX(i)] = make_float2((float)ua.V.x, (float)ua.V.y); vm[IX(i)] = ua.vm; va[IX(i)] = ua.va;
+                    if (i2 != i) { V[IX(i2)] = ub.V; Vf[IX(i2)] = make_float2((float)ub.V.x, (float)ub.V.y); vm[IX(i2)] = ub.vm; va[IX(i2)] = ub.va; }
                 }
                 // (the bus lanes above read right-hand-side blocks only; the cleared set holds the fill-in blocks)
                 PB_LOOP for (int k = tid; k < n_bzero; k += T) A4[IX(bzero[k])] = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -101,7 +101,11 @@ struct PlanHeader {
     int o_yptr, o_ynb;     // u16 [nb + 1] row pointer, u16 neighbour bus per entry
     int o_yval;            // fp64 [entries][2]: Y_ij
     int o_yblk;            // u16 per entry: block index
-    int pad2[1];
+    // the same rows packed for the kernel's bus phase (one load per entry and per bus instead of one per field):
+    int o_yword;           // u32 per entry: block index (bits 0-15) | neighbour bus (bits 16-30) | bit 31: the neighbour is a PQ bus
+    int o_yf32;            // fp32 [entries][2]: (float) of Y_ij, the operands of the off-diagonal blocks
+    int o_bdesc;           // u32 [nb][2]: {bdpos | dcidx << 16, shidx | bit 16: the bus is a PQ bus}
+    int pad2[2];
 };
 static_assert(sizeof(PlanHeader) % 16 == 0, "plan blobs are concatenated 16-byte aligned");
 
@@ -128,6 +132,7 @@ inline int plan_block_smem_bytes(int nb, int n_line, int nblkA, int n_rowcol, in
     o += (size_t)2 * n_shunt * 8;            // shunt admittance (g, b) of the buses that carry one
     o += (size_t)nb * 16;                    // V (e, f)
     o += (size_t)2 * n_line * 16;            // branch currents, both ends
+    o += (size_t)nb * 8;                     // V in fp32 (the operands of the off-diagonal blocks)
     o += ((size_t)n_rowcol * 4 + 15) & ~(size_t)15;
     return (int)((o + 15) & ~(size_t)15);
 }
@@ -821,8 +826,8 @@ public:
         H.o_brf = put_u16(brf); H.o_brt = put_u16(brt);
         if (!blk_) { H.o_round = put_u16(round); H.o_jpos = put_u16v(jpos); }
         H.o_unit_bus = put_u16(unit_bus); H.o_load_bus = put_u16(load_bus); H.o_sto_bus = put_u16(sto_bus); H.o_sh_bus = put_u16(sh_bus);
+        std::vector<int> shidx(nb, -1);
         {
-            std::vector<int> shidx(nb, -1);
             int n_shb = 0;
             for (int i = 0; i < nb; ++i) if (!bh[i].empty()) shidx[i] = n_shb++;
             H.o_shidx = put_u16(shidx); H.n_shb = n_shb;
@@ -841,6 +846,24 @@ public:
             H.o_yval = put_d(yval);
             H.o_bdpos = put_u16(bdpos); H.o_bjpos = put_u16(bjpos); H.o_bzero = put_u16(bzero); H.o_bpass_ptr = put_i32(bpass_ptr);
             H.o_yptr = put_u16(yptr); H.o_ynb = put_u16(ynb); H.o_yblk = put_u16(yblk);
+            const size_t ne = ynb.size();
+            // (at least one entry: the kernel's first round of a bus pair reads entry 0 even when both rows are empty)
+            std::vector<int> yword(ne > 0 ? ne : 1, 0), bdesc((size_t)nb * 2);
+            std::vector<float> yf32(ne > 0 ? 2 * ne : 2, 0.f);
+            for (size_t e = 0; e < ne; ++e) {
+                yword[e] = (int)((unsigned)yblk[e] | (unsigned)ynb[e] << 16 | (colv[ynb[e]] >= 0 ? 1u << 31 : 0u));
+                yf32[2 * e] = (float)yval[2 * e]; yf32[2 * e + 1] = (float)yval[2 * e + 1];
+            }
+            for (int i = 0; i < nb; ++i) {
+                bdesc[(size_t)2 * i] = (int)((bdpos[i] < 0 ? 0xFFFFu : (unsigned)bdpos[i]) | (dcidx[i] < 0 ? 0xFFFFu : (unsigned)dcidx[i]) << 16);
+                bdesc[(size_t)2 * i + 1] = (int)((shidx[i] < 0 ? 0xFFFFu : (unsigned)shidx[i]) | (colv[i] >= 0 ? 1u << 16 : 0u));
+            }
+            H.o_yword = put_i32(yword);
+            align(8);                                                  // (uint2 / float2 loads)
+            H.o_bdesc = put_i32(bdesc);
+            H.o_yf32 = (int)blob.size();
+            blob.resize(blob.size() + yf32.size() * 4);
+            if (!yf32.empty()) memcpy(&blob[H.o_yf32], yf32.data(), yf32.size() * 4);
         }
         PLAN_TICK("serialise");
         align(16);
@@ -851,7 +874,7 @@ public:
 
     // the plan format addresses values and list entries with 16 bits
     static bool fits(const PlanHeader &H) {
-        if (H.blk) return (size_t)(H.nblkA + 1) * 16 * (size_t)H.blk_G <= 0xFFFF && H.nb < 0xFFFF;
+        if (H.blk) return (size_t)(H.nblkA + 1) * 16 * (size_t)H.blk_G <= 0xFFFF && H.nb < 0x8000;
         return H.nA + 1 < 0x3FFF && H.n_op < (1 << 30);
     }
 
