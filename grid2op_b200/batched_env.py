@@ -345,16 +345,24 @@ class BatchedEnv(BatchedDoNothing):
 
     # ---- line-attack opponent ---------------------------------------------------------------------------------------------
     def enable_opponent(self, kind: str, lines_attacked, *, attack_duration: int, attack_cooldown: int, budget_per_ts: float,
-                        init_budget: float, attack_period: Optional[int] = None, rho_normalization=None, seeds):
+                        init_budget: float, attack_period: Optional[int] = None, rho_normalization=None, seeds,
+                        attack_every_xxx_hour: Optional[float] = None, average_attack_duration_hour: Optional[float] = None,
+                        minimum_attack_duration_hour: Optional[float] = None, pmax_pmin_ratio: float = 4,
+                        delta_time_seconds: float = 300.0, episode_max_time=None):
         """Give every instance grid2op's line-attack opponent (``OpponentSpace`` + ``BaseActionBudget``): ``kind``
-        ``"RandomLineOpponent"`` or ``"WeightedRandomOpponent"``; ``lines_attacked``: line names (``GridModel.name_line``) or ids;
-        the other parameters are the environment config's ``opponent_attack_duration``, ``opponent_attack_cooldown``,
-        ``opponent_budget_per_ts``, ``opponent_init_budget`` and ``kwargs_opponent`` (``attack_period``, ``rho_normalization``);
-        ``seeds``: int [B], the opponent seed of each instance (:func:`grid2op_b200.opponent.opponent_seed` of an environment
-        seed gives the one ``env.seed`` gives).  Every instance starts from ``OpponentSpace.reset()``; :meth:`reset_instances`
-        resets it again (its random stream continues).  Call it after the first step (``reset_step``): the weighted opponent reads
-        the rho of the previous step.  From then on :meth:`step` / :meth:`step_tensors` report ``info["opponent_attack_line"]``
-        (int32 [B], -1: none) and ``info["opponent_attack_duration"]`` (int32 [B])."""
+        ``"RandomLineOpponent"``, ``"WeightedRandomOpponent"`` or ``"GeometricOpponent"``; ``lines_attacked``: line names
+        (``GridModel.name_line``) or ids; the other parameters are the environment config's ``opponent_attack_duration``,
+        ``opponent_attack_cooldown``, ``opponent_budget_per_ts``, ``opponent_init_budget`` and ``kwargs_opponent``
+        (``attack_period``, ``rho_normalization``; ``attack_every_xxx_hour``, ``average_attack_duration_hour``,
+        ``minimum_attack_duration_hour``, ``pmax_pmin_ratio`` for the GeometricOpponent, with the environment's
+        ``delta_time_seconds``); ``seeds``: int [B], the opponent seed of each instance (:func:`grid2op_b200.opponent.opponent_seed`
+        of an environment seed gives the one ``env.seed`` gives).  Every instance starts from ``OpponentSpace.reset()``, the
+        GeometricOpponent with the attack schedule ``env.seed(s); env.reset()`` draws; :meth:`reset_instances` resets it again (its
+        random stream continues, a new schedule is drawn).  ``episode_max_time`` (GeometricOpponent): ``env.max_episode_duration()``,
+        an int or one per scenario of the chronics array; default: the scenarios' ``max_step`` when :meth:`enable_observation` was
+        called first, else the chronics array's row count - 1.  Call it after the first step (``reset_step``): the weighted and
+        geometric opponents read the rho of the previous step.  From then on :meth:`step` / :meth:`step_tensors` report
+        ``info["opponent_attack_line"]`` (int32 [B], -1: none) and ``info["opponent_attack_duration"]`` (int32 [B])."""
         from .opponent import BatchedOpponent
         if self.n_steps == 0:
             raise RuntimeError("enable_opponent() after the first step (reset_step): the opponent observes the previous step")
@@ -363,9 +371,19 @@ class BatchedEnv(BatchedDoNothing):
         ids = [names.index(x) if isinstance(x, str) else int(x) for x in lines_attacked]
         if any(not 0 <= l < self.gm.n_line for l in ids):
             raise ValueError("attacked line out of range")
+        geo = {}
+        if kind == "GeometricOpponent":
+            if episode_max_time is None:
+                per_scen = (self._obs["tables"]["max_step"] if self._obs is not None
+                            else np.full(self.chron.shape[0], self.chron.shape[1] - 1))
+            else:
+                per_scen = np.broadcast_to(np.asarray(episode_max_time, dtype=np.int64), (self.chron.shape[0],))
+            geo = dict(attack_every_xxx_hour=attack_every_xxx_hour, average_attack_duration_hour=average_attack_duration_hour,
+                       minimum_attack_duration_hour=minimum_attack_duration_hour, pmax_pmin_ratio=pmax_pmin_ratio,
+                       delta_time_seconds=delta_time_seconds, episode_max_time=np.asarray(per_scen, dtype=np.int64)[self.scen])
         self._opp = BatchedOpponent(kind, ids, self.batch, attack_duration=attack_duration, attack_cooldown=attack_cooldown,
                                     budget_per_ts=budget_per_ts, init_budget=init_budget, seeds=seeds, attack_period=attack_period,
-                                    rho_normalization=rho_normalization)
+                                    rho_normalization=rho_normalization, **geo)
         if self._dev is not None:
             self._opp_bind_device()
 
@@ -374,7 +392,7 @@ class BatchedEnv(BatchedDoNothing):
         o = self._opp
         if from_reset:
             return np.full(self.batch, -1, dtype=np.int32), np.zeros(self.batch, dtype=np.int32)
-        rho = self.engine.series_fetch(want_out=False)[3] if o.weighted else None        # (what the previous step wrote)
+        rho = self.engine.series_fetch(want_out=False)[3] if o.weighted or o.geometric else None    # (what the previous step wrote)
         return o.attack(self.line_status(), rho, ~self.done)
 
     def _apply_attack(self, line, dur):
@@ -395,7 +413,9 @@ class BatchedEnv(BatchedDoNothing):
     def opponent_state(self) -> dict:
         """the opponent state of every instance as the device keeps it: budget float64 [B], budget64 uint8 [B] (the budget is a
         float64 since its first charge), ctr int32 [B, 4] (attack duration, cooldown, last line, steps to the weighted opponent's
-        next attack), mt uint32 [B, 624] / mt_pos int32 [B] (the random streams)"""
+        next attack), mt uint32 [B, 624] / mt_pos int32 [B] (the random streams); a GeometricOpponent adds geo_wait / geo_dur
+        int32 [B, cap] (its attack schedules) and geo_ctr int32 [B, 4] (schedule length, attacks consumed, previous_fails, schedule
+        entries dropped at the cap: 0 unless the cap was too small)"""
         if self._opp is None:
             raise RuntimeError("call enable_opponent() first")
         self._to_host()
@@ -602,6 +622,11 @@ class BatchedEnv(BatchedDoNothing):
                                   attack_duration=int(o.attack_duration), attack_cooldown=int(o.attack_cooldown),
                                   budget_per_ts=float(o.budget_per_ts), init_budget=float(o.init_budget), mt=s["mt"], mt_pos=s["mt_pos"]),
                              d["opp_line"].data_ptr(), d["opp_dur"].data_ptr(), d["opp_budget"].data_ptr())
+        if o.geometric:
+            self.engine.opp_geo_bind(dict(weights=o.geo_weights, p_hazard=o.hazard_rate, p_recovery=o.recovery_rate,
+                                          logq_hazard=o.logq_hazard, logq_recovery=o.logq_recovery,
+                                          recovery_min=o.recovery_min, episode_max_time=o.emt, geo_wait=s["geo_wait"],
+                                          geo_dur=s["geo_dur"], geo_ctr=s["geo_ctr"]))
         self._authority = "host"              # (the next step_tensors pushes the whole state, the opponent's included)
 
     def _to_device(self):
@@ -618,7 +643,10 @@ class BatchedEnv(BatchedDoNothing):
         self.engine.env_set_state(self.topo, self._nb_inst, self._cap_dirty, self._obs["reset"] if obs else None,
                                   self.observe_inputs() if obs else None)
         if self._opp is not None:
-            self.engine.opp_set_state(self._opp.get_state())
+            s = self._opp.get_state()
+            self.engine.opp_set_state(s)
+            if self._opp.geometric:
+                self.engine.opp_geo_set_state(s)
         self._illegal_seen = self.engine.env_stats()["n_illegal"]
         self._authority = "device"
 
@@ -638,7 +666,10 @@ class BatchedEnv(BatchedDoNothing):
         if self._obs is not None:
             self._obs["reset"][:] = s["obs_reset"]
         if self._opp is not None:
-            self._opp.set_state(self.engine.opp_get_state())
+            s = self.engine.opp_get_state()
+            if self._opp.geometric:
+                s.update(self.engine.opp_geo_get_state())
+            self._opp.set_state(s)
         if self.tight_cap and self._cap_dirty.any():
             self.nb_cap = self._bus_cap()
 

@@ -124,6 +124,7 @@ struct b200pf_handle {
     // line-attack opponent of the device environment (b200pf_opp_bind)
     OppArgs opp{}; int opp_batch = 0;
     std::vector<void *> opp_allocs;
+    OppGeoArgs opp_geo{}; bool opp_geo_bound = false;            // kind OPP_GEOMETRIC (b200pf_opp_geo_bind; its buffers in opp_allocs)
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -1957,6 +1958,8 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
@@ -1973,7 +1976,7 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
         pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h));
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo);
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2029,6 +2032,8 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
 extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const int32_t *d_rows) {
     if (!h || !d_mask) return fail(B200PF_E_ARG, "null pointer");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2037,7 +2042,7 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     a.reset_mask = d_mask; a.reset_rows = d_rows;
     const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
     a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h));
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2139,7 +2144,8 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     const DevGrid &g = h->g;
-    if ((d->kind != OPP_RANDOM_LINE && d->kind != OPP_WEIGHTED_RANDOM) || d->n_attack < 1 || d->n_attack > OPP_MAX_ATTACK || !d->lines ||
+    if ((d->kind != OPP_RANDOM_LINE && d->kind != OPP_WEIGHTED_RANDOM && d->kind != OPP_GEOMETRIC) || d->n_attack < 1 ||
+        d->n_attack > OPP_MAX_ATTACK || !d->lines ||
         (d->kind == OPP_WEIGHTED_RANDOM && (!d->rho_norm || d->attack_period < 1)) || d->attack_duration < 0 || d->attack_cooldown < 0 ||
         !d->mt || !d->mt_pos || !d->attack_line || !d->attack_dur || !d->budget)
         return fail(B200PF_E_ARG, "bad opponent description");
@@ -2151,6 +2157,7 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
     for (void *p : h->opp_allocs) cudaFree(p);
     h->opp_allocs.clear();
     h->opp_batch = 0;
+    h->opp_geo = OppGeoArgs{}; h->opp_geo_bound = false;
     auto dev = [&](const void *src, size_t bytes, void **dst) -> int {
         CU(cudaMalloc(dst, bytes));
         h->opp_allocs.push_back(*dst);
@@ -2218,6 +2225,72 @@ extern "C" int b200pf_opp_set_state(b200pf_handle *h, const double *budget, cons
     if (mt_pos) H2D(o.mt_pos, mt_pos, B * 4);
     CU(cudaStreamSynchronize(h->stream));
     h->env_h2d += (int64_t)((budget ? B * 8 : 0) + (budget64 ? B : 0) + (ctr ? B * OPP_CTR * 4 : 0) + (mt ? B * OPP_MT_N * 4 : 0) + (mt_pos ? B * 4 : 0));
+    return 0;
+}
+
+extern "C" int b200pf_opp_geo_bind(b200pf_handle *h, const b200pf_opp_geo_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!opp_bound(h) || h->opp.kind != OPP_GEOMETRIC) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_bind, kind 3)");
+    if (!d->weights || !d->episode_max_time || !d->wait || !d->dur || !d->gctr || d->cap < 1 || d->recovery_min < 0 ||
+        !(d->p_hazard > 0.0 && d->p_hazard <= 1.0) || !(d->p_recovery > 0.0 && d->p_recovery <= 1.0))
+        return fail(B200PF_E_ARG, "bad GeometricOpponent description");
+    const int B = h->opp_batch;
+    for (int i = 0; i < B; ++i) {
+        const int32_t *gc = d->gctr + (size_t)i * OPP_GEO_CTR;
+        if (gc[OPP_GEO_N] < 0 || gc[OPP_GEO_N] > d->cap || gc[OPP_GEO_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
+    }
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    const size_t n_sched = (size_t)B * (size_t)d->cap * 4;
+    void *p[5] = {};
+    const void *src[5] = {d->weights, d->episode_max_time, d->wait, d->dur, d->gctr};
+    const size_t bytes[5] = {(size_t)h->opp.n_attack * 8, (size_t)B * 4, n_sched, n_sched, (size_t)B * OPP_GEO_CTR * 4};
+    for (int k = 0; k < 5; ++k) {
+        CU(cudaMalloc(&p[k], bytes[k]));
+        h->opp_allocs.push_back(p[k]);
+        H2D(p[k], src[k], bytes[k]);
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    OppGeoArgs g{};
+    g.weights = (const double *)p[0]; g.p_hazard = d->p_hazard; g.p_recovery = d->p_recovery;
+    g.logq_hazard = d->logq_hazard; g.logq_recovery = d->logq_recovery; g.recovery_min = d->recovery_min; g.cap = d->cap;
+    g.emt = (const int32_t *)p[1]; g.wait = (int32_t *)p[2]; g.dur = (int32_t *)p[3]; g.gctr = (int32_t *)p[4];
+    h->opp_geo = g; h->opp_geo_bound = true;
+    return 0;
+}
+
+static bool opp_geo_ready(const b200pf_handle *h) { return opp_bound(h) && h->opp.kind == OPP_GEOMETRIC && h->opp_geo_bound; }
+
+extern "C" int b200pf_opp_geo_get_state(b200pf_handle *h, int32_t *wait, int32_t *dur, int32_t *gctr) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_geo_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_geo_bind)");
+    CU(cudaSetDevice(h->device));
+    const OppGeoArgs &g = h->opp_geo;
+    const size_t B = (size_t)h->opp_batch, n_sched = B * (size_t)g.cap * 4;
+    CU(cudaStreamSynchronize(h->stream));
+    if (wait) CU(cudaMemcpy(wait, g.wait, n_sched, cudaMemcpyDeviceToHost));
+    if (dur) CU(cudaMemcpy(dur, g.dur, n_sched, cudaMemcpyDeviceToHost));
+    if (gctr) CU(cudaMemcpy(gctr, g.gctr, B * OPP_GEO_CTR * 4, cudaMemcpyDeviceToHost));
+    h->env_d2h += (int64_t)((wait ? n_sched : 0) + (dur ? n_sched : 0) + (gctr ? B * OPP_GEO_CTR * 4 : 0));
+    return 0;
+}
+
+extern "C" int b200pf_opp_geo_set_state(b200pf_handle *h, const int32_t *wait, const int32_t *dur, const int32_t *gctr) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_geo_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_geo_bind)");
+    const OppGeoArgs &g = h->opp_geo;
+    const size_t B = (size_t)h->opp_batch, n_sched = B * (size_t)g.cap * 4;
+    if (gctr)
+        for (size_t i = 0; i < B; ++i) {
+            const int32_t *gc = gctr + i * OPP_GEO_CTR;
+            if (gc[OPP_GEO_N] < 0 || gc[OPP_GEO_N] > g.cap || gc[OPP_GEO_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
+        }
+    CU(cudaSetDevice(h->device));
+    if (wait) H2D(g.wait, wait, n_sched);
+    if (dur) H2D(g.dur, dur, n_sched);
+    if (gctr) H2D(g.gctr, gctr, B * OPP_GEO_CTR * 4);
+    CU(cudaStreamSynchronize(h->stream));
+    h->env_h2d += (int64_t)((wait ? n_sched : 0) + (dur ? n_sched : 0) + (gctr ? B * OPP_GEO_CTR * 4 : 0));
     return 0;
 }
 

@@ -123,7 +123,8 @@ ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
 }
 
 // BatchedEnv._apply_agent followed by _apply_environment and the opponent's attack (o: NULL or no opponent bound), for instance i
-ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr) {
+// (g: the GeometricOpponent's part, NULL for the other kinds)
+ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr) {
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * a.dim_topo;
@@ -136,7 +137,7 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     // the opponent decides first, on the line status the previous step left (grid2op's current_obs); its attack lands last
     int opp_line = -1, opp_dur = 0;
     if (o && o->kind != OPP_NONE) {
-        if (!done && !a.from_reset) opp_line = opp_decide_instance(*o, i, tv, a.line_or_pos, a.line_ex_pos, nl, &opp_dur);
+        if (!done && !a.from_reset) opp_line = opp_decide_instance(*o, i, tv, a.line_or_pos, a.line_ex_pos, nl, &opp_dur, g);
         o->attack_line[i] = opp_line; o->attack_dur[i] = opp_dur;
     }
     if (!a.from_reset) {
@@ -320,9 +321,10 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i) {
 }
 
 // BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
-ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr) {
+ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr) {
     if (!a.reset_mask[i]) return;
     if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
+    if (o && g && o->kind == OPP_GEOMETRIC) opp_geo_reset_instance(*o, *g, i);
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const int8_t *t0v = a.topo0 + (size_t)i * a.n_topo_in;
@@ -365,10 +367,10 @@ __global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a) {
 }
 
 // one thread per instance; nothing is written when the validation flagged an input
-__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o) {
+__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.batch || *(volatile int32_t *)&a.ctl[ENV_CTL_ERR]) return;
-    env_apply_instance(a, i, &o);
+    env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
@@ -376,9 +378,9 @@ __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
     if (i < a.batch) env_post_instance(a, i);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_reset_instance(a, i, &o);
+    if (i < a.batch) env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

@@ -1,17 +1,20 @@
 // b200pf_opp.cuh — line-attack opponents of BatchedEnv for a whole batch on the device: grid2op's OpponentSpace with
-// BaseActionBudget and a RandomLineOpponent or a WeightedRandomOpponent, restated per instance, with each instance's own
-// numpy-legacy random stream (RandomState: MT19937 and its legacy draws).
+// BaseActionBudget and a RandomLineOpponent, a WeightedRandomOpponent or a GeometricOpponent, restated per instance, with each
+// instance's own numpy-legacy random stream (RandomState: MT19937 and its legacy draws).
 //
 // The body restates grid2op_b200/opponent.py (the numpy reference path) in the same order:
-//   opp_decide_instance   OpponentSpace.attack and the opponent's attack / tell_attack_continues, on the line status and rho
-//                         the previous step left;
-//   opp_reset_instance    OpponentSpace.reset (the random stream is not reseeded: it continues).
+//   opp_decide_instance     OpponentSpace.attack and the opponent's attack / tell_attack_continues, on the line status and rho
+//                           the previous step left;
+//   opp_reset_instance      OpponentSpace.reset (the random stream is not reseeded: it continues);
+//   opp_geo_reset_instance  the GeometricOpponent's part of it: a new attack schedule (sample_attack_times_and_durations).
+// The GeometricOpponent's constants and schedules are an OppGeoArgs next to OppArgs (NULL for the other kinds).
 // env_apply_instance (b200pf_env.cuh) calls the first before the agent's action and applies the attack after the environment's
 // own outages; env_reset_instance calls the second.  The bodies are __host__ __device__: the CUDA launches run one thread per
 // instance, a host build (tests/emu/opp_emu.cpp) runs the same source over the batch.  The fp64 arithmetic of the weighted draw is
 // written with explicitly rounded operations (no contraction), so both builds round as numpy does.
 #pragma once
 
+#include <cmath>
 #include <cstddef>
 #include <cstdint>
 
@@ -23,11 +26,27 @@
 
 namespace b200pf {
 
-enum { OPP_NONE = 0, OPP_RANDOM_LINE = 1, OPP_WEIGHTED_RANDOM = 2 };
+enum { OPP_NONE = 0, OPP_RANDOM_LINE = 1, OPP_WEIGHTED_RANDOM = 2, OPP_GEOMETRIC = 3 };
 enum { OPP_MT_N = 624, OPP_MAX_ATTACK = 64 };
 // per-instance counters, int32 [batch][OPP_CTR]
 enum { OPP_CTR_DURATION = 0, OPP_CTR_COOLDOWN = 1, OPP_CTR_LAST = 2, OPP_CTR_NEXT = 3, OPP_CTR = 4 };
-static const int32_t OPP_NEXT_UNSET = INT32_MIN;    // WeightedRandomOpponent._next_attack_time is None
+static const int32_t OPP_NEXT_UNSET = INT32_MIN;    // WeightedRandomOpponent / GeometricOpponent._next_attack_time is None
+// per-instance counters of the GeometricOpponent, int32 [batch][OPP_GEO_CTR]: attacks in the schedule, attacks consumed,
+// OpponentSpace.previous_fails, schedules that did not fit the cap (their tail was drawn and dropped)
+enum { OPP_GEO_N = 0, OPP_GEO_COUNTER = 1, OPP_GEO_FAILS = 2, OPP_GEO_OVERFLOW = 3, OPP_GEO_CTR = 4 };
+
+// GeometricOpponent (kind OPP_GEOMETRIC): its constants and its schedule state, next to OppArgs (whose ctr[OPP_CTR_NEXT] is its
+// _next_attack_time)
+struct OppGeoArgs {
+    const double *weights;                          // [n_attack] np.exp(b_beta * k), k = 0 .. n_attack - 1 (computed by numpy)
+    double p_hazard, p_recovery;                    // p of the geometric waiting times / of the random part of the durations
+    double logq_hazard, logq_recovery;              // log(1 - p) of both (the inversion's divisor, computed on the host)
+    int recovery_min;                               // _recovery_minimum_duration
+    int cap;                                        // schedule entries per instance
+    const int32_t *emt;                             // [batch] _episode_max_time
+    int32_t *wait, *dur;                            // [batch][cap] _attack_waiting_times, _attack_durations
+    int32_t *gctr;                                  // [batch][OPP_GEO_CTR]
+};
 
 struct OppArgs {
     int kind;                                       // OPP_NONE: no opponent bound
@@ -139,6 +158,94 @@ OPP_HD inline int opp_choice_weighted(uint32_t *mt, int32_t *pos, const double *
     return idx;
 }
 
+// geometric(p) (numpy's legacy_random_geometric): for p >= 1/3 the search on one random_sample(), else the inversion
+// ceil(log1p(-U) / log(1 - p)) with logq = log(1 - p).  log1p is CUDA's on the device (within 1 ulp) and libm's in a host build;
+// the quotient is rounded up to an integer, so a last-bit difference changes the draw only when it lies within an ulp or two of an
+// integer (DESIGN §7 f.1).  The search stops where numpy would loop forever (the running product underflowed: its sum cannot grow).
+OPP_HD inline int64_t opp_geometric(uint32_t *mt, int32_t *pos, double p, double logq) {
+    if (p >= 0.333333333333333333333333) {
+        const double q = opp_dadd(1.0, -p);
+        const double u = opp_random_sample(mt, pos);
+        double sum = p, prod = p;
+        int64_t x = 1;
+        while (u > sum && prod > 0.0) { prod = opp_dmul(prod, q); sum = opp_dadd(sum, prod); ++x; }
+        return x;
+    }
+    return (int64_t)ceil(opp_ddiv(log1p(-opp_random_sample(mt, pos)), logq));
+}
+
+// ---- GeometricOpponent ----------------------------------------------------------------------------------------------------
+// sample_attack_times_and_durations for instance i, on its stream: waiting times and durations until episode_max_time.  Entries past
+// the cap are drawn (the stream stays grid2op's) but dropped and counted in OPP_GEO_OVERFLOW.
+OPP_HD inline void opp_geo_sample(const OppGeoArgs &g, int i, uint32_t *mt, int32_t *pos) {
+    int32_t *w = g.wait + (size_t)i * g.cap, *d = g.dur + (size_t)i * g.cap;
+    int32_t *gc = g.gctr + (size_t)i * OPP_GEO_CTR;
+    const int64_t emt = g.emt[i];
+    int64_t t = 0;
+    int n = 0;
+    while (t < emt) {
+        const int64_t tw = opp_geometric(mt, pos, g.p_hazard, g.logq_hazard);
+        t += tw;
+        if (t < emt) {
+            const int64_t td = (int64_t)g.recovery_min + opp_geometric(mt, pos, g.p_recovery, g.logq_recovery);
+            if (n < g.cap) { w[n] = (int32_t)tw; d[n] = (int32_t)td; ++n; }
+            else gc[OPP_GEO_OVERFLOW] += 1;
+            t += td;
+        }
+    }
+    gc[OPP_GEO_N] = n; gc[OPP_GEO_COUNTER] = 0; gc[OPP_GEO_FAILS] = 0;
+}
+
+// GeometricOpponent.attack for instance i -> the attacked line (-1: none); *dur: its duration from the schedule
+OPP_HD inline int opp_geo_attack(const OppArgs &o, const OppGeoArgs &g, int i, const int8_t *tv, const int32_t *line_or_pos,
+                                 const int32_t *line_ex_pos, int n_line, int32_t *ctr, int32_t *gc, int *dur) {
+    const int c = gc[OPP_GEO_COUNTER], n = gc[OPP_GEO_N];
+    if (c >= n) return -1;                                                             // no attack left in the schedule
+    const int32_t *w = g.wait + (size_t)i * g.cap, *d = g.dur + (size_t)i * g.cap;
+    // (int32 sums wrap as numpy's do; d[-1] of a failure before any attack is numpy's last entry)
+    if (gc[OPP_GEO_FAILS]) ctr[OPP_CTR_NEXT] = (int32_t)((uint32_t)w[c] + (uint32_t)d[c > 0 ? c - 1 : n - 1]);
+    if (ctr[OPP_CTR_NEXT] == OPP_NEXT_UNSET) ctr[OPP_CTR_NEXT] = (int32_t)(1u + (uint32_t)w[c]);
+    *dur = d[c];
+    ctr[OPP_CTR_NEXT] -= 1;
+    if (ctr[OPP_CTR_NEXT] > 0) return -1;
+    gc[OPP_GEO_COUNTER] = c + 1;                                                       // the attack is consumed, whatever follows
+    for (int k = 0; k < o.n_attack; ++k) {                                             // ~status.all(): one line out -> no attack
+        const int l = o.lines[k];
+        if (!(tv[line_or_pos[l]] > 0 && tv[line_ex_pos[l]] > 0)) return -1;
+    }
+    if (o.n_attack == 1) return o.lines[0];
+    // Boltzmann weights on the rho ranks: rank k = lines with a lower rho, ties ranked by line order (a stable argsort)
+    const float *rho = o.rho + (size_t)i * n_line;
+    double wv[OPP_MAX_ATTACK];
+    for (int k = 0; k < o.n_attack; ++k) {
+        const float r = rho[o.lines[k]];
+        int rank = 0;
+        for (int j = 0; j < o.n_attack; ++j) {
+            const float rj = rho[o.lines[j]];
+            rank += (rj < r || (rj == r && j < k)) ? 1 : 0;
+        }
+        wv[k] = g.weights[rank];
+    }
+    const double s = opp_np_sum(wv, o.n_attack);
+    return o.lines[opp_choice_weighted(o.mt + (size_t)i * OPP_MT_N, o.mt_pos + i, wv, o.n_attack, s)];
+}
+
+// OpponentSpace.attack's call of the geometric opponent with its checks: refused (and previous_fails set) when the opponent's duration
+// exceeds attack_max_duration or duration * cost exceeds the budget b; previous_fails is cleared otherwise
+OPP_HD inline int opp_geo_asked(const OppArgs &o, const OppGeoArgs &g, int i, const int8_t *tv, const int32_t *line_or_pos,
+                                const int32_t *line_ex_pos, int n_line, int32_t *ctr, double b) {
+    int32_t *gc = g.gctr + (size_t)i * OPP_GEO_CTR;
+    int d = 0;
+    int attack = opp_geo_attack(o, g, i, tv, line_or_pos, line_ex_pos, n_line, ctr, gc, &d);
+    const int duration = attack >= 0 ? d : o.attack_duration;                          // None -> attack_max_duration
+    bool fails = false;
+    if (duration > o.attack_duration) { attack = -1; fails = true; }
+    if ((attack >= 0 ? (double)duration : 0.0) > b) { attack = -1; fails = true; }     // duration * cost > budget
+    gc[OPP_GEO_FAILS] = fails ? 1 : 0;
+    if (attack >= 0) { ctr[OPP_CTR_DURATION] = duration; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
+    return attack;
+}
+
 // ---- the opponent ---------------------------------------------------------------------------------------------------------
 // The opponent's choice among the attackable lines that are connected in ``tv`` (the topology the previous step left): -1 for none.
 OPP_HD inline int opp_choose(const OppArgs &o, int i, const int8_t *tv, const int32_t *line_or_pos, const int32_t *line_ex_pos,
@@ -168,7 +275,7 @@ OPP_HD inline int opp_choose(const OppArgs &o, int i, const int8_t *tv, const in
 
 // OpponentSpace.attack for instance i (not finished, not a reset step) -> the attacked line (-1: none); *dur: its duration
 OPP_HD inline int opp_decide_instance(const OppArgs &o, int i, const int8_t *tv, const int32_t *line_or_pos, const int32_t *line_ex_pos,
-                                      int n_line, int *dur) {
+                                      int n_line, int *dur, const OppGeoArgs *g = nullptr) {
     int32_t *ctr = o.ctr + (size_t)i * OPP_CTR;
     double b = o.budget[i];
     const bool b64 = o.budget64[i] != 0;
@@ -180,12 +287,17 @@ OPP_HD inline int opp_decide_instance(const OppArgs &o, int i, const int8_t *tv,
     if (ctr[OPP_CTR_DURATION] > 0) attack = ctr[OPP_CTR_LAST];                           // the running attack continues
     else if (ctr[OPP_CTR_COOLDOWN] <= o.attack_cooldown) {
         asked = true;
-        attack = opp_choose(o, i, tv, line_or_pos, line_ex_pos, n_line, ctr);
-        // duration None -> attack_max_duration; the cost of one line is 1: refused when duration * cost > budget
-        if (attack >= 0 && (double)o.attack_duration > b) attack = -1;
-        if (attack >= 0) { ctr[OPP_CTR_DURATION] = o.attack_duration; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
+        if (o.kind == OPP_GEOMETRIC) {
+            if (g) attack = opp_geo_asked(o, *g, i, tv, line_or_pos, line_ex_pos, n_line, ctr, b);
+        } else {
+            attack = opp_choose(o, i, tv, line_or_pos, line_ex_pos, n_line, ctr);
+            // duration None -> attack_max_duration; the cost of one line is 1: refused when duration * cost > budget
+            if (attack >= 0 && (double)o.attack_duration > b) attack = -1;
+            if (attack >= 0) { ctr[OPP_CTR_DURATION] = o.attack_duration; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
+        }
     }
-    if (!asked && o.kind == OPP_WEIGHTED_RANDOM) ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;      // tell_attack_continues
+    if (!asked && o.kind != OPP_RANDOM_LINE) ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;        // tell_attack_continues
+    if (!asked && g) g->gctr[(size_t)i * OPP_GEO_CTR + OPP_GEO_FAILS] = 0;               // (OpponentSpace clears previous_fails)
     ctr[OPP_CTR_LAST] = attack;
     if (attack >= 0) { b = b - 1.0; o.budget64[i] = 1; }                                    // budget -= cost: float32 - int64 -> float64
     o.budget[i] = b;
@@ -198,6 +310,11 @@ OPP_HD inline void opp_reset_instance(const OppArgs &o, int i) {
     int32_t *ctr = o.ctr + (size_t)i * OPP_CTR;
     o.budget[i] = (double)o.init_budget; o.budget64[i] = 0;
     ctr[OPP_CTR_DURATION] = 0; ctr[OPP_CTR_COOLDOWN] = o.attack_cooldown; ctr[OPP_CTR_LAST] = -1; ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;
+}
+
+// OpponentSpace.reset's GeometricOpponent.reset for instance i: a new schedule from the continuing stream
+OPP_HD inline void opp_geo_reset_instance(const OppArgs &o, const OppGeoArgs &g, int i) {
+    opp_geo_sample(g, i, o.mt + (size_t)i * OPP_MT_N, o.mt_pos + i);
 }
 
 }  // namespace b200pf

@@ -40,6 +40,7 @@ ABI_SYMBOLS = (
     "b200pf_last_launch_config", "b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state",
     "b200pf_env_set_state", "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats",
     "b200pf_opp_bind", "b200pf_opp_get_state", "b200pf_opp_set_state",
+    "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
 )
 
 
@@ -97,6 +98,15 @@ class OppDesc(C.Structure):
         ("kind", C.c_int32), ("n_attack", C.c_int32), ("lines", C.c_void_p), ("rho_norm", C.c_void_p), ("attack_period", C.c_int32),
         ("attack_duration", C.c_int32), ("attack_cooldown", C.c_int32), ("budget_per_ts", C.c_float), ("init_budget", C.c_float),
         ("mt", C.c_void_p), ("mt_pos", C.c_void_p), ("attack_line", C.c_void_p), ("attack_dur", C.c_void_p), ("budget", C.c_void_p),
+    ]
+
+
+class OppGeoDesc(C.Structure):
+    """``b200pf_opp_geo_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("weights", C.c_void_p), ("p_hazard", C.c_double), ("p_recovery", C.c_double), ("logq_hazard", C.c_double),
+        ("logq_recovery", C.c_double), ("recovery_min", C.c_int32), ("cap", C.c_int32), ("episode_max_time", C.c_void_p),
+        ("wait", C.c_void_p), ("dur", C.c_void_p), ("gctr", C.c_void_p),
     ]
 
 
@@ -260,9 +270,12 @@ def load_library():
     lib.b200pf_opp_bind.argtypes = [vp, C.POINTER(OppDesc)]
     lib.b200pf_opp_get_state.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.b200pf_opp_set_state.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.b200pf_opp_geo_bind.argtypes = [vp, C.POINTER(OppGeoDesc)]
+    lib.b200pf_opp_geo_get_state.argtypes = [vp, vp, vp, vp]
+    lib.b200pf_opp_geo_set_state.argtypes = [vp, vp, vp, vp]
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
-               "b200pf_opp_set_state"):
+               "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -747,6 +760,33 @@ class PowerFlowEngine:
         a = [np.ascontiguousarray(s[k], dt) for k, dt in (("budget", np.float64), ("budget64", np.uint8), ("ctr", np.int32),
                                                             ("mt", np.uint32), ("mt_pos", np.int32))]
         self._check(self.lib.b200pf_opp_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_set_state")
+
+    def opp_geo_bind(self, t: dict):
+        """the GeometricOpponent's constants and first schedules (``b200pf_opp_geo_bind``, after ``opp_bind`` with kind 3): ``t``
+        built by BatchedEnv.enable_opponent"""
+        keep = [np.ascontiguousarray(t["weights"], np.float64), np.ascontiguousarray(t["episode_max_time"], np.int32),
+                np.ascontiguousarray(t["geo_wait"], np.int32), np.ascontiguousarray(t["geo_dur"], np.int32),
+                np.ascontiguousarray(t["geo_ctr"], np.int32)]
+        cap = int(keep[2].shape[1])
+        d = OppGeoDesc(weights=keep[0].ctypes.data, p_hazard=float(t["p_hazard"]), p_recovery=float(t["p_recovery"]),
+                       logq_hazard=float(t["logq_hazard"]), logq_recovery=float(t["logq_recovery"]), recovery_min=int(t["recovery_min"]),
+                       cap=cap, episode_max_time=keep[1].ctypes.data, wait=keep[2].ctypes.data, dur=keep[3].ctypes.data,
+                       gctr=keep[4].ctypes.data)
+        self._check(self.lib.b200pf_opp_geo_bind(self.h, C.byref(d)), "b200pf_opp_geo_bind")
+        self._opp_geo_cap = cap
+        del keep
+
+    def opp_geo_get_state(self):
+        """-> dict(geo_wait int32 [B, cap], geo_dur int32 [B, cap], geo_ctr int32 [B, 4]) of the GeometricOpponent"""
+        B, cap = self._series_batch, getattr(self, "_opp_geo_cap", 0)       # (unbound: the library refuses the call)
+        s = dict(geo_wait=np.empty((B, cap), np.int32), geo_dur=np.empty((B, cap), np.int32), geo_ctr=np.empty((B, 4), np.int32))
+        self._check(self.lib.b200pf_opp_geo_get_state(self.h, *[_ptr(s[k]) for k in ("geo_wait", "geo_dur", "geo_ctr")]),
+                    "b200pf_opp_geo_get_state")
+        return s
+
+    def opp_geo_set_state(self, s: dict):
+        a = [np.ascontiguousarray(s[k], np.int32) for k in ("geo_wait", "geo_dur", "geo_ctr")]
+        self._check(self.lib.b200pf_opp_geo_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_geo_set_state")
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")

@@ -6,7 +6,13 @@ Restates, per instance, grid2op's ``OpponentSpace`` (grid2op/Opponent/opponentSp
 
 * ``RandomLineOpponent`` (randomLineOpponent.py): a uniform choice among the connected attackable lines;
 * ``WeightedRandomOpponent`` (weightedRandomOpponent.py): the attack time is drawn uniformly within ``attack_period`` steps, the
-  line with ``p = rho / rho_normalization / sum`` among the connected attackable lines.
+  line with ``p = rho / rho_normalization / sum`` among the connected attackable lines;
+* ``GeometricOpponent`` (geometricOpponent.py): at every reset it draws a schedule for the whole episode, geometric waiting times
+  and durations (``RandomState.geometric``); an attack whose time has come is consumed, and lands only when every attackable line
+  is connected (grid2op's ``~status.all()`` test), on a line drawn with Boltzmann weights ``exp(b_beta * rank)`` of the lines'
+  rho ranks, for the schedule's duration.  OpponentSpace refuses it (and sets ``previous_fails``, which moves the next attack) when
+  that duration exceeds ``attack_duration`` or the budget.  Ranks of equal rho follow the line order (a stable argsort): numpy's
+  default argsort is not stable for ties on every host, so that is the one place the reference's own choice can differ.
 
 Each instance has its own ``np.random.RandomState`` (the opponent's ``space_prng``).  The arithmetic below is numpy's own, on
 numpy scalars, as the reference does it: the budget is a float32 until the first charge (float32 - int64 promotes it to float64
@@ -23,11 +29,40 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-__all__ = ["OPPONENT_KINDS", "BatchedOpponent", "opponent_seed", "NEXT_UNSET"]
+__all__ = ["OPPONENT_KINDS", "BatchedOpponent", "opponent_seed", "geometric_constants", "NEXT_UNSET"]
 
-OPPONENT_KINDS = {"RandomLineOpponent": 1, "WeightedRandomOpponent": 2}
-NEXT_UNSET = -2 ** 31                  # WeightedRandomOpponent._next_attack_time is None (device encoding)
+OPPONENT_KINDS = {"RandomLineOpponent": 1, "WeightedRandomOpponent": 2, "GeometricOpponent": 3}
+NEXT_UNSET = -2 ** 31                  # WeightedRandomOpponent / GeometricOpponent._next_attack_time is None (device encoding)
 _COST = np.int64(1)                    # BaseActionBudget of one line's set_line_status action
+_INT32_MAX = 2 ** 31 - 1
+_LOG_U_MAX = float(np.log(2.0 ** -53))  # log1p(-U) for the largest random_sample(), 1 - 2**-53: the largest geometric draw
+
+
+def _max_geometric(p: float) -> int:
+    """about the largest value ``RandomState.geometric(p)`` can return, ``0 < p <= 1``"""
+    return 1 if p >= 1.0 else int(np.ceil(_LOG_U_MAX / np.log1p(-p))) + 1
+
+
+def geometric_constants(attack_every_xxx_hour, average_attack_duration_hour, minimum_attack_duration_hour, delta_time_seconds=300.0):
+    """``GeometricOpponent.init``'s rates: -> (recovery_min int, recovery_rate, attack_hazard_rate); its OpponentError cases and rates
+    whose draws would not fit an int32 (grid2op's ``astype(dt_int)`` would wrap them) raise ValueError.  The environment's
+    ``delta_time_seconds`` is a float32, so the steps per hour and both rates are float32 values, as in grid2op."""
+    ts_per_hour = 3600.0 / np.float32(delta_time_seconds)
+    recovery_min = int(minimum_attack_duration_hour * ts_per_hour)
+    if average_attack_duration_hour < minimum_attack_duration_hour:
+        raise ValueError("The average duration of an attack cannot be lower than the minimum time of an attack")
+    if average_attack_duration_hour == minimum_attack_duration_hour:
+        raise ValueError("average_attack_duration_hour == minimum_attack_duration_hour is not supported")
+    recovery_rate = 1.0 / (ts_per_hour * (average_attack_duration_hour - minimum_attack_duration_hour))
+    if attack_every_xxx_hour <= average_attack_duration_hour:
+        raise ValueError("attack_every_xxx_hour <= average_attack_duration_hour is not supported")
+    hazard_rate = 1.0 / (ts_per_hour * (attack_every_xxx_hour - average_attack_duration_hour))
+    for name, p, extra in (("attack hazard", hazard_rate, 0), ("recovery", recovery_rate, recovery_min)):
+        if not 0.0 < p <= 1.0:
+            raise ValueError(f"the {name} rate {p} is not a probability (fewer than one step per hour?)")
+        if recovery_min < 0 or extra + _max_geometric(float(p)) > _INT32_MAX:
+            raise ValueError(f"the {name} rate {p} is too small: its draws would not fit an int32")
+    return recovery_min, recovery_rate, hazard_rate
 
 
 def opponent_seed(env_seed: int) -> int:
@@ -46,7 +81,12 @@ class BatchedOpponent:
 
     def __init__(self, kind: str, lines: Sequence[int], batch: int, *, attack_duration: int, attack_cooldown: int,
                  budget_per_ts: float, init_budget: float, seeds, attack_period: Optional[int] = None,
-                 rho_normalization: Optional[Sequence[float]] = None):
+                 rho_normalization: Optional[Sequence[float]] = None, attack_every_xxx_hour: Optional[float] = None,
+                 average_attack_duration_hour: Optional[float] = None, minimum_attack_duration_hour: Optional[float] = None,
+                 pmax_pmin_ratio: float = 4, delta_time_seconds: float = 300.0, episode_max_time=None):
+        """``GeometricOpponent``: ``attack_every_xxx_hour``, ``average_attack_duration_hour``, ``minimum_attack_duration_hour``,
+        ``pmax_pmin_ratio`` (its ``kwargs_opponent``), ``delta_time_seconds`` (the environment's step) and ``episode_max_time`` (int
+        or int [batch]: ``env.max_episode_duration()`` of each instance's scenario)."""
         if kind not in OPPONENT_KINDS:
             raise ValueError(f"unknown opponent {kind!r} ({' / '.join(OPPONENT_KINDS)})")
         self.kind = kind
@@ -82,7 +122,57 @@ class BatchedOpponent:
         self.cooldown = np.zeros(batch, dtype=np.int64)
         self.last = np.full(batch, -1, dtype=np.int64)
         self.next_time = [None] * batch
+        self.geometric = kind == "GeometricOpponent"
+        if self.geometric:
+            self._init_geometric(attack_every_xxx_hour, average_attack_duration_hour, minimum_attack_duration_hour, pmax_pmin_ratio,
+                                 delta_time_seconds, episode_max_time)
         self.reset(np.arange(batch))
+
+    def _init_geometric(self, every, average, minimum, pmax_pmin_ratio, delta_time_seconds, episode_max_time):
+        if every is None or average is None or minimum is None:
+            raise ValueError("GeometricOpponent needs attack_every_xxx_hour, average_attack_duration_hour and minimum_attack_duration_hour")
+        if not float(pmax_pmin_ratio) > 0.0:
+            raise ValueError("pmax_pmin_ratio must be > 0")
+        if not float(delta_time_seconds) > 0.0:
+            raise ValueError("delta_time_seconds must be > 0")
+        self.recovery_min, self.recovery_rate, self.hazard_rate = geometric_constants(every, average, minimum, delta_time_seconds)
+        # the divisor of numpy's inversion, log(1 - p) in double precision (RandomState.geometric takes p as a double)
+        self.logq_hazard, self.logq_recovery = float(np.log(1.0 - float(self.hazard_rate))), float(np.log(1.0 - float(self.recovery_rate)))
+        if episode_max_time is None:
+            raise ValueError("GeometricOpponent needs episode_max_time")
+        emt = np.broadcast_to(np.asarray(episode_max_time, dtype=np.int64), (self.batch,))
+        if (emt < 0).any() or (emt > _INT32_MAX).any():
+            raise ValueError("episode_max_time out of range")
+        self.emt = emt.astype(np.int32)
+        self.pmax_pmin_ratio = pmax_pmin_ratio
+        n = len(self.lines)
+        # GeometricOpponent.attack's expressions, for every rank at once: the lines it weighs are always all attackable lines
+        self.b_beta = np.log(pmax_pmin_ratio) / (n - 1) if n > 1 else np.float64(0.0)
+        self.geo_weights = np.exp(self.b_beta * np.arange(n, dtype=np.int64))
+        # every appended attack advances the schedule's time by at least recovery_min + 2 (a wait >= 1, a duration >= recovery_min + 1)
+        self.cap = int(-(-int(self.emt.max()) // (self.recovery_min + 2))) + 1
+        self.geo_wait = np.zeros((self.batch, self.cap), dtype=np.int32)
+        self.geo_dur = np.zeros((self.batch, self.cap), dtype=np.int32)
+        self.geo_ctr = np.zeros((self.batch, 4), dtype=np.int32)         # schedule length, attacks consumed, previous_fails, dropped
+
+    def _geo_sample(self, i):
+        """GeometricOpponent.sample_attack_times_and_durations"""
+        rng, emt = self.rngs[i], int(self.emt[i])
+        waits, durs = [], []
+        t = 0
+        while t < emt:
+            t_to_attack = rng.geometric(p=self.hazard_rate)
+            t = t + t_to_attack
+            if t < emt:
+                waits.append(t_to_attack)
+                d = self.recovery_min + rng.geometric(p=self.recovery_rate)
+                durs.append(d)
+                t = t + d
+        n = min(len(waits), self.cap)
+        self.geo_wait[i, :n] = np.array(waits[:n]).astype(np.int32)
+        self.geo_dur[i, :n] = np.array(durs[:n]).astype(np.int32)
+        self.geo_ctr[i, 0], self.geo_ctr[i, 1], self.geo_ctr[i, 2] = n, 0, 0
+        self.geo_ctr[i, 3] += len(waits) - n
 
     # ---- OpponentSpace.reset ----------------------------------------------------------------------------------------------
     def reset(self, idx):
@@ -93,6 +183,8 @@ class BatchedOpponent:
             self.cooldown[i] = int(self.attack_cooldown)
             self.last[i] = -1
             self.next_time[i] = None
+            if self.geometric:
+                self._geo_sample(int(i))
 
     # ---- OpponentSpace.attack ---------------------------------------------------------------------------------------------
     def attack(self, line_status: np.ndarray, rho: Optional[np.ndarray], live: np.ndarray):
@@ -120,13 +212,22 @@ class BatchedOpponent:
             attack, duration = self._opponent_attack(i, status, rho)
             if duration is None:
                 duration = self.attack_duration
-            if duration * self._cost(attack) > self.budget[i]:
+            if self.geometric:
+                fails = False
+                if duration > self.attack_duration:
+                    attack, fails = None, True
+                if duration * self._cost(attack) > self.budget[i]:
+                    attack, fails = None, True
+                self.geo_ctr[i, 2] = fails                                  # previous_fails
+            elif duration * self._cost(attack) > self.budget[i]:
                 attack = None
             if attack is not None:
                 self.duration[i] = duration
                 self.cooldown[i] += self.attack_cooldown
-        if not asked and self.weighted:
+        if not asked and (self.weighted or self.geometric):
             self.next_time[i] = None                                        # tell_attack_continues
+        if not asked and self.geometric:
+            self.geo_ctr[i, 2] = 0
         self.budget[i] = self.budget[i] - self._cost(attack)
         self.last[i] = -1 if attack is None else attack
         return (-1, 0) if attack is None else (attack, int(self.duration[i]))
@@ -135,8 +236,39 @@ class BatchedOpponent:
     def _cost(attack):
         return 0 if attack is None else _COST
 
+    def _geo_attack(self, i, status, rho):
+        """GeometricOpponent.attack"""
+        rng = self.rngs[i]
+        n, c = int(self.geo_ctr[i, 0]), int(self.geo_ctr[i, 1])
+        if c >= n:
+            return None, None
+        wait, dur = self.geo_wait[i, :n], self.geo_dur[i, :n]
+        if self.geo_ctr[i, 2]:
+            self.next_time[i] = wait[c] + dur[c - 1]
+        if self.next_time[i] is None:
+            self.next_time[i] = 1 + wait[c]
+        attack_duration = dur[c]
+        self.next_time[i] -= 1
+        if self.next_time[i] > 0:
+            return None, None
+        self.geo_ctr[i, 1] = c + 1
+        st = np.asarray(status, dtype=bool)[self.lines]
+        if ~st.all():
+            return None, None
+        if len(self.lines) == 1:
+            return int(self.lines[0]), attack_duration
+        r = np.asarray(rho, dtype=np.float32)[self.lines]
+        temp = r.argsort(kind="stable")
+        rho_ranks = np.empty_like(temp)
+        rho_ranks[temp] = np.arange(len(r))
+        raw_probabilities = np.exp(self.b_beta * rho_ranks)
+        b_probabilities = raw_probabilities / raw_probabilities.sum()
+        return int(rng.choice(self.lines, p=b_probabilities)), attack_duration
+
     def _opponent_attack(self, i, status, rho):
         rng = self.rngs[i]
+        if self.geometric:
+            return self._geo_attack(i, status, rho)
         if self.weighted:
             if self.next_time[i] is None:
                 self.next_time[i] = 1 + rng.randint(self.attack_period)
@@ -157,7 +289,9 @@ class BatchedOpponent:
 
     # ---- the state as the device keeps it (b200pf_opp_get_state / b200pf_opp_set_state) ------------------------------------
     def get_state(self):
-        """-> dict(budget float64 [B], budget64 uint8 [B], ctr int32 [B, 4], mt uint32 [B, 624], mt_pos int32 [B])"""
+        """-> dict(budget float64 [B], budget64 uint8 [B], ctr int32 [B, 4], mt uint32 [B, 624], mt_pos int32 [B]); a
+        GeometricOpponent adds geo_wait / geo_dur int32 [B, cap] (the schedules) and geo_ctr int32 [B, 4] (schedule length, attacks
+        consumed, previous_fails, schedule entries dropped at the cap)"""
         B = self.batch
         ctr = np.empty((B, 4), dtype=np.int32)
         ctr[:, 0], ctr[:, 1], ctr[:, 2] = self.duration, self.cooldown, self.last
@@ -167,12 +301,19 @@ class BatchedOpponent:
         for i, r in enumerate(self.rngs):
             st = r.get_state()
             mt[i], pos[i] = st[1], st[2]
-        return dict(budget=np.array([float(b) for b in self.budget], dtype=np.float64),
-                    budget64=np.array([b.dtype == np.float64 for b in self.budget], dtype=np.uint8), ctr=ctr, mt=mt, mt_pos=pos)
+        s = dict(budget=np.array([float(b) for b in self.budget], dtype=np.float64),
+                 budget64=np.array([b.dtype == np.float64 for b in self.budget], dtype=np.uint8), ctr=ctr, mt=mt, mt_pos=pos)
+        if self.geometric:
+            s.update(geo_wait=self.geo_wait.copy(), geo_dur=self.geo_dur.copy(), geo_ctr=self.geo_ctr.copy())
+        return s
 
     def set_state(self, s):
         for i in range(self.batch):
             self.budget[i] = np.float64(s["budget"][i]) if s["budget64"][i] else np.float32(s["budget"][i])
             self.rngs[i].set_state(("MT19937", np.asarray(s["mt"][i], dtype=np.uint32), int(s["mt_pos"][i]), 0, 0.0))
         self.duration[:], self.cooldown[:], self.last[:] = s["ctr"][:, 0], s["ctr"][:, 1], s["ctr"][:, 2]
-        self.next_time = [None if int(t) == NEXT_UNSET else int(t) for t in s["ctr"][:, 3]]
+        if self.geometric:              # (grid2op keeps _next_attack_time as a numpy int32)
+            self.next_time = [None if int(t) == NEXT_UNSET else np.int32(t) for t in s["ctr"][:, 3]]
+            self.geo_wait[:], self.geo_dur[:], self.geo_ctr[:] = s["geo_wait"], s["geo_dur"], s["geo_ctr"]
+        else:
+            self.next_time = [None if int(t) == NEXT_UNSET else int(t) for t in s["ctr"][:, 3]]

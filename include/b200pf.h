@@ -404,7 +404,7 @@ int b200pf_env_stats(const b200pf_handle *h, int64_t *out8);
  * duration, current attack cooldown, last attacked line or -1, steps to the weighted opponent's next attack or INT32_MIN for
  * none), mt uint32 [batch][624] and mt_pos int32 [batch].  Unbound (b200pf_opp_bind never called), nothing of the above runs. */
 typedef struct b200pf_opp_desc {
-    int32_t kind;                       /* 1: RandomLineOpponent, 2: WeightedRandomOpponent */
+    int32_t kind;                       /* 1: RandomLineOpponent, 2: WeightedRandomOpponent, 3: GeometricOpponent */
     int32_t n_attack;                   /* attackable lines, 1..64 */
     const int32_t *lines;               /* [n_attack] their line ids */
     const double *rho_norm;             /* [n_attack] rho normalisation (kind 2) */
@@ -421,6 +421,27 @@ int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *desc);
 int b200pf_opp_get_state(b200pf_handle *h, double *budget, uint8_t *budget64, int32_t *ctr, uint32_t *mt, int32_t *mt_pos);
 int b200pf_opp_set_state(b200pf_handle *h, const double *budget, const uint8_t *budget64, const int32_t *ctr, const uint32_t *mt,
                          const int32_t *mt_pos);
+
+/* GeometricOpponent (kind 3): b200pf_opp_bind with kind 3 (rho_norm and attack_period unused), then b200pf_opp_geo_bind with its
+ * constants and every instance's first schedule; b200pf_env_step refuses to step a kind-3 opponent without it.  Each instance keeps
+ * an attack schedule (waiting times and durations int32 [cap], drawn by GeometricOpponent.sample_attack_times_and_durations with
+ * RandomState.geometric on the instance's stream) and four int32 counters: schedule length, attacks consumed, OpponentSpace's
+ * previous_fails, and schedule entries dropped because they did not fit the cap (0 unless cap is too small).  ctr[3] of
+ * b200pf_opp_get_state is the opponent's _next_attack_time (INT32_MIN for None).  b200pf_env_reset draws a new schedule for each
+ * reset instance on the device.  The apply launch reads the rho the previous step left, as for kind 2. */
+typedef struct b200pf_opp_geo_desc {
+    const double *weights;              /* [n_attack] np.exp(b_beta * k), k = 0 .. n_attack - 1 */
+    double p_hazard, p_recovery;        /* attack hazard rate, recovery rate */
+    double logq_hazard, logq_recovery;  /* log(1 - p) of both */
+    int32_t recovery_min;               /* minimum attack duration in steps */
+    int32_t cap;                        /* schedule entries per instance, >= 1 */
+    const int32_t *episode_max_time;    /* [batch] */
+    const int32_t *wait, *dur;          /* [batch][cap] the initial schedules */
+    const int32_t *gctr;                /* [batch][4] their counters */
+} b200pf_opp_geo_desc;
+int b200pf_opp_geo_bind(b200pf_handle *h, const b200pf_opp_geo_desc *desc);
+int b200pf_opp_geo_get_state(b200pf_handle *h, int32_t *wait, int32_t *dur, int32_t *gctr);
+int b200pf_opp_geo_set_state(b200pf_handle *h, const int32_t *wait, const int32_t *dur, const int32_t *gctr);
 
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */

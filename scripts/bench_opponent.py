@@ -1,8 +1,9 @@
 """BatchedEnv.step_tensors with and without the line-attack opponent (enable_opponent), alternating in one process, on the workloads
 of scripts/bench_env_tensor.py: random one-substation and one-line actions drawn on the GPU with a seeded torch generator, then
 observe, finished instances reset on the device; protections off and on; case14 at batch 4096 (RandomLineOpponent on the lines of
-rte_case14_opponent) and l2rpn_neurips_2020_track1 at batch 1024 (its WeightedRandomOpponent).  The opponents use their environments'
-constants with a small initial budget, so that attacks run from the first steps on.  A host clock around K steps that end in a device
+rte_case14_opponent), l2rpn_neurips_2020_track1 at batch 1024 (its WeightedRandomOpponent) and l2rpn_wcci_2022_dev at batch 1024
+(its GeometricOpponent, with the environment's own constants: its device resets draw a new attack schedule).  The first two use their
+environments' constants with a small initial budget, so that attacks run from the first steps on.  A host clock around K steps that end in a device
 synchronise, after warm-up.  Prints env.step/s (min / median / max over the repeats), the extra bytes per step the opponent moves, and
 the card and its power limit read in the same run.
 
@@ -28,6 +29,14 @@ OPPONENTS = {
                                              "44_45_126", "34_35_110", "54_58_154"],
                                       rho_normalization=[0.45, 0.45, 0.6, 0.35, 0.3, 0.2, 0.55, 0.3, 0.45, 0.55], attack_period=12,
                                       attack_duration=48, attack_cooldown=288, budget_per_ts=0.16667, init_budget=48.0),
+    # the environment's own GeometricOpponent (config.py): attacks every 24 h on average, 4 h long, at least 1 h
+    "l2rpn_wcci_2022_dev": dict(kind="GeometricOpponent",
+                                lines=["26_31_106", "21_22_93", "17_18_88", "4_10_162", "12_14_68", "14_32_108", "62_58_180", "62_63_160",
+                                       "48_50_136", "48_53_141", "41_48_131", "39_41_121", "43_44_125", "44_45_126", "34_35_110",
+                                       "54_58_154", "74_117_81", "80_79_175", "93_95_43", "88_91_33", "91_92_37", "99_105_62",
+                                       "102_104_61"],
+                                attack_duration=96, attack_cooldown=12, budget_per_ts=0.17, init_budget=144.0, attack_every_xxx_hour=24,
+                                average_attack_duration_hour=4, minimum_attack_duration_hour=1),
 }
 
 
@@ -105,7 +114,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=5)
     args = ap.parse_args()
     print("card, power limit:", card())
-    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024)):
+    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024), ("l2rpn_wcci_2022_dev", 1024)):
         for prot in (False, True):
             run(name, B, prot, args.steps, args.warmup, args.repeats)
 
