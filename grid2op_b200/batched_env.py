@@ -362,17 +362,27 @@ class BatchedEnv(BatchedDoNothing):
         an int or one per scenario of the chronics array; default: the scenarios' ``max_step`` when :meth:`enable_observation` was
         called first, else the chronics array's row count - 1.  Call it after the first step (``reset_step``): the weighted and
         geometric opponents read the rho of the previous step.  From then on :meth:`step` / :meth:`step_tensors` report
-        ``info["opponent_attack_line"]`` (int32 [B], -1: none) and ``info["opponent_attack_duration"]`` (int32 [B])."""
+        ``info["opponent_attack_line"]`` (int32 [B], -1: none) and ``info["opponent_attack_duration"]`` (int32 [B]).
+
+        ``"GeometricOpponentMultiArea"`` (l2rpn_idf_2023): ``lines_attacked`` is a list of areas (lists of names or ids), at most 8
+        areas and 64 lines, no line in two areas; the other arguments are the GeometricOpponent's, and ``attack_cooldown`` must be 0
+        or 1.  Each area is a GeometricOpponent with its own stream (seeded from the instance's seed as ``env.seed`` seeds it) and
+        schedule; ``info["opponent_attack_line"]`` is then int32 [B, n_area], each area's line in the step's attack (-1: none), and
+        ``info["opponent_attack_duration"]`` is 1 where an attack landed."""
         from .opponent import BatchedOpponent
         if self.n_steps == 0:
             raise RuntimeError("enable_opponent() after the first step (reset_step): the opponent observes the previous step")
         self._to_host()
         names = list(getattr(self.gm, "name_line", []))
-        ids = [names.index(x) if isinstance(x, str) else int(x) for x in lines_attacked]
-        if any(not 0 <= l < self.gm.n_line for l in ids):
-            raise ValueError("attacked line out of range")
+
+        def line_ids(group):
+            ids = [names.index(x) if isinstance(x, str) else int(x) for x in group]
+            if any(not 0 <= l < self.gm.n_line for l in ids):
+                raise ValueError("attacked line out of range")
+            return ids
+        ids = [line_ids(a) for a in lines_attacked] if kind == "GeometricOpponentMultiArea" else line_ids(lines_attacked)
         geo = {}
-        if kind == "GeometricOpponent":
+        if kind in ("GeometricOpponent", "GeometricOpponentMultiArea"):
             if episode_max_time is None:
                 per_scen = (self._obs["tables"]["max_step"] if self._obs is not None
                             else np.full(self.chron.shape[0], self.chron.shape[1] - 1))
@@ -391,16 +401,19 @@ class BatchedEnv(BatchedDoNothing):
         """OpponentSpace.attack of the live instances (none on a reset step) -> (line int32 [B], duration int32 [B])"""
         o = self._opp
         if from_reset:
-            return np.full(self.batch, -1, dtype=np.int32), np.zeros(self.batch, dtype=np.int32)
-        rho = self.engine.series_fetch(want_out=False)[3] if o.weighted or o.geometric else None    # (what the previous step wrote)
+            line = np.full((self.batch, len(o.area_off) - 1) if o.multi else self.batch, -1, dtype=np.int32)
+            return line, np.zeros(self.batch, dtype=np.int32)
+        rho = (self.engine.series_fetch(want_out=False)[3] if o.weighted or o.geometric or o.multi
+               else None)                                                   # (what the previous step wrote)
         return o.attack(self.line_status(), rho, ~self.done)
 
     def _apply_attack(self, line, dur):
-        """the attacked lines are out (both ends), their cooldown at least the attack's duration"""
-        ii = np.flatnonzero(line >= 0)
+        """the attacked lines are out (both ends), their cooldown at least the attack's duration (``line`` [B] or, several lines
+        per instance, [B, n])"""
+        ii, kk = np.nonzero(line.reshape(self.batch, -1) >= 0)
         if not len(ii):
             return
-        ll = line[ii].astype(np.int64)
+        ll = line.reshape(self.batch, -1)[ii, kk].astype(np.int64)
         lc = self.line_cooldown
         lc[ii, ll] = np.maximum(lc[ii, ll], dur[ii])
         was_on = (self.topo[ii, self.line_or_pos[ll]] > 0) | (self.topo[ii, self.line_ex_pos[ll]] > 0)
@@ -415,7 +428,8 @@ class BatchedEnv(BatchedDoNothing):
         float64 since its first charge), ctr int32 [B, 4] (attack duration, cooldown, last line, steps to the weighted opponent's
         next attack), mt uint32 [B, 624] / mt_pos int32 [B] (the random streams); a GeometricOpponent adds geo_wait / geo_dur
         int32 [B, cap] (its attack schedules) and geo_ctr int32 [B, 4] (schedule length, attacks consumed, previous_fails, schedule
-        entries dropped at the cap: 0 unless the cap was too small)"""
+        entries dropped at the cap: 0 unless the cap was too small); a GeometricOpponentMultiArea adds multi_mt / multi_mt_pos,
+        multi_wait / multi_dur, multi_ctr and multi_fails (:meth:`grid2op_b200.opponent.BatchedOpponent.get_state`)"""
         if self._opp is None:
             raise RuntimeError("call enable_opponent() first")
         self._to_host()
@@ -614,6 +628,7 @@ class BatchedEnv(BatchedDoNothing):
     def _opp_bind_device(self):
         """the opponent's constants and initial random states to the device; its per-step outputs are device buffers of ours"""
         import torch
+        from .opponent import MULTI_KEYS
         d, o, B = self._dev, self._opp, self.batch
         z = lambda dt: torch.zeros(B, dtype=dt, device=d["device"])           # noqa: E731
         d["opp_line"], d["opp_dur"], d["opp_budget"] = z(torch.int32), z(torch.int32), z(torch.float64)
@@ -627,6 +642,12 @@ class BatchedEnv(BatchedDoNothing):
                                           logq_hazard=o.logq_hazard, logq_recovery=o.logq_recovery,
                                           recovery_min=o.recovery_min, episode_max_time=o.emt, geo_wait=s["geo_wait"],
                                           geo_dur=s["geo_dur"], geo_ctr=s["geo_ctr"]))
+        if o.multi:
+            d["opp_lines"] = torch.full((B, len(o.area_off) - 1), -1, dtype=torch.int32, device=d["device"])
+            self.engine.opp_multi_bind(dict(area_off=o.area_off, weights=o.area_weights, p_hazard=o.hazard_rate,
+                                            p_recovery=o.recovery_rate, logq_hazard=o.logq_hazard, logq_recovery=o.logq_recovery,
+                                            recovery_min=o.recovery_min, episode_max_time=o.emt, **{k: s[k] for k in MULTI_KEYS}),
+                                       d["opp_lines"].data_ptr())
         self._authority = "host"              # (the next step_tensors pushes the whole state, the opponent's included)
 
     def _to_device(self):
@@ -647,6 +668,8 @@ class BatchedEnv(BatchedDoNothing):
             self.engine.opp_set_state(s)
             if self._opp.geometric:
                 self.engine.opp_geo_set_state(s)
+            if self._opp.multi:
+                self.engine.opp_multi_set_state(s)
         self._illegal_seen = self.engine.env_stats()["n_illegal"]
         self._authority = "device"
 
@@ -669,6 +692,8 @@ class BatchedEnv(BatchedDoNothing):
             s = self.engine.opp_get_state()
             if self._opp.geometric:
                 s.update(self.engine.opp_geo_get_state())
+            if self._opp.multi:
+                s.update(self.engine.opp_multi_get_state())
             self._opp.set_state(s)
         if self.tight_cap and self._cap_dirty.any():
             self.nb_cap = self._bus_cap()
@@ -734,7 +759,8 @@ class BatchedEnv(BatchedDoNothing):
         info = {"status": d["status"], "iters": d["iters"], "newly_done": d["newly_done"], "is_illegal": d["is_illegal"],
                 "disc_lines": d["disc"] if self.protections else None}
         if self._opp is not None:
-            info["opponent_attack_line"], info["opponent_attack_duration"] = d["opp_line"], d["opp_dur"]
+            info["opponent_attack_line"] = d["opp_lines"] if self._opp.multi else d["opp_line"]
+            info["opponent_attack_duration"] = d["opp_dur"]
         return d["rho"], d["done"], info
 
     def _reset_tensors(self, mask, rows=None):

@@ -125,6 +125,7 @@ struct b200pf_handle {
     OppArgs opp{}; int opp_batch = 0;
     std::vector<void *> opp_allocs;
     OppGeoArgs opp_geo{}; bool opp_geo_bound = false;            // kind OPP_GEOMETRIC (b200pf_opp_geo_bind; its buffers in opp_allocs)
+    OppMultiArgs opp_multi{}; bool opp_multi_bound = false;      // kind OPP_GEOMETRIC_MULTI (b200pf_opp_multi_bind; likewise)
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -1960,6 +1961,8 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
         return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
@@ -1976,7 +1979,7 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
         pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo);
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi);
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2034,6 +2037,8 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
         return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2042,7 +2047,7 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     a.reset_mask = d_mask; a.reset_rows = d_rows;
     const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
     a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo);
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2144,7 +2149,8 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     const DevGrid &g = h->g;
-    if ((d->kind != OPP_RANDOM_LINE && d->kind != OPP_WEIGHTED_RANDOM && d->kind != OPP_GEOMETRIC) || d->n_attack < 1 ||
+    if ((d->kind != OPP_RANDOM_LINE && d->kind != OPP_WEIGHTED_RANDOM && d->kind != OPP_GEOMETRIC && d->kind != OPP_GEOMETRIC_MULTI) ||
+        d->n_attack < 1 ||
         d->n_attack > OPP_MAX_ATTACK || !d->lines ||
         (d->kind == OPP_WEIGHTED_RANDOM && (!d->rho_norm || d->attack_period < 1)) || d->attack_duration < 0 || d->attack_cooldown < 0 ||
         !d->mt || !d->mt_pos || !d->attack_line || !d->attack_dur || !d->budget)
@@ -2158,6 +2164,7 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
     h->opp_allocs.clear();
     h->opp_batch = 0;
     h->opp_geo = OppGeoArgs{}; h->opp_geo_bound = false;
+    h->opp_multi = OppMultiArgs{}; h->opp_multi_bound = false;
     auto dev = [&](const void *src, size_t bytes, void **dst) -> int {
         CU(cudaMalloc(dst, bytes));
         h->opp_allocs.push_back(*dst);
@@ -2291,6 +2298,96 @@ extern "C" int b200pf_opp_geo_set_state(b200pf_handle *h, const int32_t *wait, c
     if (gctr) H2D(g.gctr, gctr, B * OPP_GEO_CTR * 4);
     CU(cudaStreamSynchronize(h->stream));
     h->env_h2d += (int64_t)((wait ? n_sched : 0) + (dur ? n_sched : 0) + (gctr ? B * OPP_GEO_CTR * 4 : 0));
+    return 0;
+}
+
+// the per-area arrays of a GeometricOpponentMultiArea: MT words, MT positions, waiting times, durations, counters, previous_fails
+static void opp_multi_sizes(const OppMultiArgs &m, size_t B, size_t out[6]) {
+    const size_t ba = B * (size_t)m.n_area;
+    out[0] = ba * OPP_MT_N * 4; out[1] = ba * 4; out[2] = out[3] = ba * (size_t)m.cap * 4; out[4] = ba * OPP_AREA_CTR * 4; out[5] = B * 4;
+}
+
+static int opp_multi_check(const int32_t *mt_pos, const int32_t *actr, int cap, size_t ba) {
+    for (size_t k = 0; mt_pos && k < ba; ++k)
+        if (mt_pos[k] < 0 || mt_pos[k] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
+    for (size_t k = 0; actr && k < ba; ++k) {
+        const int32_t *ac = actr + k * OPP_AREA_CTR;
+        if (ac[OPP_AREA_N] < 0 || ac[OPP_AREA_N] > cap || ac[OPP_AREA_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
+    }
+    return 0;
+}
+
+extern "C" int b200pf_opp_multi_bind(b200pf_handle *h, const b200pf_opp_multi_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!opp_bound(h) || h->opp.kind != OPP_GEOMETRIC_MULTI)
+        return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_bind, kind 4)");
+    if (d->n_area < 1 || d->n_area > OPP_MAX_AREA || !d->area_off || !d->weights || !d->episode_max_time || !d->mt || !d->mt_pos ||
+        !d->wait || !d->dur || !d->actr || !d->fails || !d->attack_lines || d->cap < 1 || d->recovery_min < 0 ||
+        !(d->p_hazard > 0.0 && d->p_hazard <= 1.0) || !(d->p_recovery > 0.0 && d->p_recovery <= 1.0))
+        return fail(B200PF_E_ARG, "bad GeometricOpponentMultiArea description");
+    if (d->area_off[0] != 0 || d->area_off[d->n_area] != h->opp.n_attack) return fail(B200PF_E_ARG, "areas do not cover the attacked lines");
+    for (int k = 0; k < d->n_area; ++k)
+        if (d->area_off[k + 1] <= d->area_off[k]) return fail(B200PF_E_ARG, "empty area");
+    const int B = h->opp_batch;
+    int rc = opp_multi_check(d->mt_pos, d->actr, d->cap, (size_t)B * d->n_area);
+    if (rc) return rc;
+    OppMultiArgs m{};
+    m.n_area = d->n_area;
+    for (int k = 0; k <= d->n_area; ++k) m.area_off[k] = d->area_off[k];
+    m.p_hazard = d->p_hazard; m.p_recovery = d->p_recovery; m.logq_hazard = d->logq_hazard; m.logq_recovery = d->logq_recovery;
+    m.recovery_min = d->recovery_min; m.cap = d->cap; m.attack_lines = d->attack_lines;
+    size_t sz[6];
+    opp_multi_sizes(m, (size_t)B, sz);
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    void *p[8] = {};
+    const void *src[8] = {d->weights, d->episode_max_time, d->mt, d->mt_pos, d->wait, d->dur, d->actr, d->fails};
+    const size_t bytes[8] = {(size_t)h->opp.n_attack * 8, (size_t)B * 4, sz[0], sz[1], sz[2], sz[3], sz[4], sz[5]};
+    for (int k = 0; k < 8; ++k) {
+        CU(cudaMalloc(&p[k], bytes[k]));
+        h->opp_allocs.push_back(p[k]);
+        H2D(p[k], src[k], bytes[k]);
+    }
+    CU(cudaStreamSynchronize(h->stream));
+    m.weights = (const double *)p[0]; m.emt = (const int32_t *)p[1]; m.mt = (uint32_t *)p[2]; m.mt_pos = (int32_t *)p[3];
+    m.wait = (int32_t *)p[4]; m.dur = (int32_t *)p[5]; m.actr = (int32_t *)p[6]; m.fails = (int32_t *)p[7];
+    h->opp_multi = m; h->opp_multi_bound = true;
+    return 0;
+}
+
+static bool opp_multi_ready(const b200pf_handle *h) { return opp_bound(h) && h->opp.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound; }
+
+extern "C" int b200pf_opp_multi_get_state(b200pf_handle *h, uint32_t *mt, int32_t *mt_pos, int32_t *wait, int32_t *dur, int32_t *actr,
+                                          int32_t *fails) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_multi_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_multi_bind)");
+    CU(cudaSetDevice(h->device));
+    const OppMultiArgs &m = h->opp_multi;
+    size_t sz[6];
+    opp_multi_sizes(m, (size_t)h->opp_batch, sz);
+    void *dst[6] = {mt, mt_pos, wait, dur, actr, fails};
+    const void *src[6] = {m.mt, m.mt_pos, m.wait, m.dur, m.actr, m.fails};
+    CU(cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < 6; ++k)
+        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
+    return 0;
+}
+
+extern "C" int b200pf_opp_multi_set_state(b200pf_handle *h, const uint32_t *mt, const int32_t *mt_pos, const int32_t *wait, const int32_t *dur,
+                                          const int32_t *actr, const int32_t *fails) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!opp_multi_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_multi_bind)");
+    const OppMultiArgs &m = h->opp_multi;
+    int rc = opp_multi_check(mt_pos, actr, m.cap, (size_t)h->opp_batch * m.n_area);
+    if (rc) return rc;
+    size_t sz[6];
+    opp_multi_sizes(m, (size_t)h->opp_batch, sz);
+    void *dst[6] = {m.mt, m.mt_pos, m.wait, m.dur, m.actr, m.fails};
+    const void *src[6] = {mt, mt_pos, wait, dur, actr, fails};
+    CU(cudaSetDevice(h->device));
+    for (int k = 0; k < 6; ++k)
+        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
+    CU(cudaStreamSynchronize(h->stream));
     return 0;
 }
 

@@ -123,8 +123,9 @@ ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
 }
 
 // BatchedEnv._apply_agent followed by _apply_environment and the opponent's attack (o: NULL or no opponent bound), for instance i
-// (g: the GeometricOpponent's part, NULL for the other kinds)
-ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr) {
+// (g: the GeometricOpponent's part, m: the GeometricOpponentMultiArea's; NULL for the other kinds)
+ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
+                                      const OppMultiArgs *m = nullptr) {
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * a.dim_topo;
@@ -137,7 +138,8 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     // the opponent decides first, on the line status the previous step left (grid2op's current_obs); its attack lands last
     int opp_line = -1, opp_dur = 0;
     if (o && o->kind != OPP_NONE) {
-        if (!done && !a.from_reset) opp_line = opp_decide_instance(*o, i, tv, a.line_or_pos, a.line_ex_pos, nl, &opp_dur, g);
+        if (!done && !a.from_reset) opp_line = opp_decide_instance(*o, i, tv, a.line_or_pos, a.line_ex_pos, nl, &opp_dur, g, m);
+        else if (m) opp_multi_none(*m, i);
         o->attack_line[i] = opp_line; o->attack_dur[i] = opp_dur;
     }
     if (!a.from_reset) {
@@ -233,12 +235,17 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
             tv[po] = -1; tv[pe] = -1;
         }
     }
-    if (opp_line >= 0) {                                      // the attack: the line is out, its cooldown at least the attack's duration
+    if (opp_line >= 0) {                                      // the attack: its lines are out, their cooldown at least its duration
         int32_t *lc = a.line_cd + (size_t)i * nl;
-        if (lc[opp_line] < opp_dur) lc[opp_line] = opp_dur;
-        const int po = a.line_or_pos[opp_line], pe = a.line_ex_pos[opp_line];
-        if (tv[po] > 0 || tv[pe] > 0) dirty = true;
-        tv[po] = -1; tv[pe] = -1;
+        const int n_hit = m ? m->n_area : 1;
+        for (int k = 0; k < n_hit; ++k) {
+            const int l = m ? m->attack_lines[(size_t)i * m->n_area + k] : opp_line;
+            if (l < 0) continue;
+            if (lc[l] < opp_dur) lc[l] = opp_dur;
+            const int po = a.line_or_pos[l], pe = a.line_ex_pos[l];
+            if (tv[po] > 0 || tv[pe] > 0) dirty = true;
+            tv[po] = -1; tv[pe] = -1;
+        }
     }
     if (dirty) { a.cap_dirty[i] = 1; ENV_ATOMIC_ADD(&a.ctl[ENV_CTL_N_DIRTY], 1); }
     if (dirty || a.stale[i]) {                                // rows the host's plan mirror has not seen
@@ -321,10 +328,12 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i) {
 }
 
 // BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
-ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr) {
+ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
+                                      const OppMultiArgs *m = nullptr) {
     if (!a.reset_mask[i]) return;
     if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
     if (o && g && o->kind == OPP_GEOMETRIC) opp_geo_reset_instance(*o, *g, i);
+    if (o && m && o->kind == OPP_GEOMETRIC_MULTI) opp_multi_reset_instance(*m, i);
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const int8_t *t0v = a.topo0 + (size_t)i * a.n_topo_in;
@@ -367,10 +376,10 @@ __global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a) {
 }
 
 // one thread per instance; nothing is written when the validation flagged an input
-__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g) {
+__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.batch || *(volatile int32_t *)&a.ctl[ENV_CTL_ERR]) return;
-    env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr);
+    env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
@@ -378,9 +387,9 @@ __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
     if (i < a.batch) env_post_instance(a, i);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr);
+    if (i < a.batch) env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

@@ -6,8 +6,10 @@
 //   opp_decide_instance     OpponentSpace.attack and the opponent's attack / tell_attack_continues, on the line status and rho
 //                           the previous step left;
 //   opp_reset_instance      OpponentSpace.reset (the random stream is not reseeded: it continues);
-//   opp_geo_reset_instance  the GeometricOpponent's part of it: a new attack schedule (sample_attack_times_and_durations).
-// The GeometricOpponent's constants and schedules are an OppGeoArgs next to OppArgs (NULL for the other kinds).
+//   opp_geo_reset_instance  the GeometricOpponent's part of it: a new attack schedule (sample_attack_times_and_durations);
+//   opp_multi_reset_instance  the GeometricOpponentMultiArea's part: a new schedule per area, in area order.
+// The GeometricOpponent's constants and schedules are an OppGeoArgs next to OppArgs (NULL for the other kinds); the
+// GeometricOpponentMultiArea's, one GeometricOpponent per area with its own stream, are an OppMultiArgs.
 // env_apply_instance (b200pf_env.cuh) calls the first before the agent's action and applies the attack after the environment's
 // own outages; env_reset_instance calls the second.  The bodies are __host__ __device__: the CUDA launches run one thread per
 // instance, a host build (tests/emu/opp_emu.cpp) runs the same source over the batch.  The fp64 arithmetic of the weighted draw is
@@ -26,7 +28,7 @@
 
 namespace b200pf {
 
-enum { OPP_NONE = 0, OPP_RANDOM_LINE = 1, OPP_WEIGHTED_RANDOM = 2, OPP_GEOMETRIC = 3 };
+enum { OPP_NONE = 0, OPP_RANDOM_LINE = 1, OPP_WEIGHTED_RANDOM = 2, OPP_GEOMETRIC = 3, OPP_GEOMETRIC_MULTI = 4 };
 enum { OPP_MT_N = 624, OPP_MAX_ATTACK = 64 };
 // per-instance counters, int32 [batch][OPP_CTR]
 enum { OPP_CTR_DURATION = 0, OPP_CTR_COOLDOWN = 1, OPP_CTR_LAST = 2, OPP_CTR_NEXT = 3, OPP_CTR = 4 };
@@ -46,6 +48,44 @@ struct OppGeoArgs {
     const int32_t *emt;                             // [batch] _episode_max_time
     int32_t *wait, *dur;                            // [batch][cap] _attack_waiting_times, _attack_durations
     int32_t *gctr;                                  // [batch][OPP_GEO_CTR]
+};
+
+// GeometricOpponentMultiArea (kind OPP_GEOMETRIC_MULTI): per-area counters, int32 [batch][n_area][OPP_AREA_CTR].  The schedule
+// length, attacks consumed and entries dropped at the cap sit where OPP_GEO_CTR has them, so both kinds share the schedule code; then
+// the area's GeometricOpponent._next_attack_time (OPP_NEXT_UNSET: None), its _new_attack_time_counters entry and its
+// _previous_attacks line (-1: None).
+enum { OPP_AREA_N = 0, OPP_AREA_COUNTER = 1, OPP_AREA_NEXT = 2, OPP_AREA_OVERFLOW = 3, OPP_AREA_CLOCK = 4, OPP_AREA_PREV = 5,
+       OPP_AREA_CTR = 6 };
+static_assert((int)OPP_AREA_N == (int)OPP_GEO_N && (int)OPP_AREA_COUNTER == (int)OPP_GEO_COUNTER &&
+              (int)OPP_AREA_OVERFLOW == (int)OPP_GEO_OVERFLOW, "the schedule code reads both layouts");
+enum { OPP_MAX_AREA = 8 };
+
+// The GeometricOpponentMultiArea: its areas (ranges of OppArgs.lines), their weight tables, the shared constants and every area's
+// stream and schedule.  OppArgs keeps OpponentSpace's part (budget, duration, cooldown; ctr[OPP_CTR_LAST] is the first line of the
+// landed attack, ctr[OPP_CTR_NEXT] stays OPP_NEXT_UNSET); previous_fails is here.
+struct OppMultiArgs {
+    int n_area;
+    int area_off[OPP_MAX_AREA + 1];                 // area k's lines are OppArgs.lines[area_off[k] .. area_off[k + 1])
+    const double *weights;                          // [n_attack] area k's np.exp(b_beta_k * r) at area_off[k] + r (computed by numpy)
+    double p_hazard, p_recovery;                    // as OppGeoArgs (every area has the same)
+    double logq_hazard, logq_recovery;
+    int recovery_min;
+    int cap;                                        // schedule entries per instance and area
+    const int32_t *emt;                             // [batch] _episode_max_time
+    uint32_t *mt; int32_t *mt_pos;                  // [batch][n_area][624], [batch][n_area]: each area's RandomState
+    int32_t *wait, *dur;                            // [batch][n_area][cap]
+    int32_t *actr;                                  // [batch][n_area][OPP_AREA_CTR]
+    int32_t *fails;                                 // [batch] OpponentSpace.previous_fails
+    int32_t *attack_lines;                          // [batch][n_area] per-step output, caller-owned: area k's line in the landed
+                                                    // attack, -1 where the area put none in it
+};
+
+// one GeometricOpponent's stream and schedule: MT state [624] and position, waiting times and durations [cap], and counters laid out
+// as OPP_GEO_CTR's schedule length, attacks consumed and dropped entries
+struct OppGeoSched {
+    uint32_t *mt; int32_t *pos;
+    int32_t *wait, *dur;
+    int32_t *gc;
 };
 
 struct OppArgs {
@@ -175,59 +215,75 @@ OPP_HD inline int64_t opp_geometric(uint32_t *mt, int32_t *pos, double p, double
 }
 
 // ---- GeometricOpponent ----------------------------------------------------------------------------------------------------
-// sample_attack_times_and_durations for instance i, on its stream: waiting times and durations until episode_max_time.  Entries past
-// the cap are drawn (the stream stays grid2op's) but dropped and counted in OPP_GEO_OVERFLOW.
-OPP_HD inline void opp_geo_sample(const OppGeoArgs &g, int i, uint32_t *mt, int32_t *pos) {
-    int32_t *w = g.wait + (size_t)i * g.cap, *d = g.dur + (size_t)i * g.cap;
-    int32_t *gc = g.gctr + (size_t)i * OPP_GEO_CTR;
-    const int64_t emt = g.emt[i];
+// sample_attack_times_and_durations on one stream and schedule: waiting times and durations until emt.  Entries past the cap are
+// drawn (the stream stays grid2op's) but dropped and counted in OPP_GEO_OVERFLOW.
+OPP_HD inline void opp_geo_draw_schedule(const OppGeoSched &s, int64_t emt, double p_hazard, double logq_hazard, double p_recovery,
+                                         double logq_recovery, int recovery_min, int cap) {
     int64_t t = 0;
     int n = 0;
     while (t < emt) {
-        const int64_t tw = opp_geometric(mt, pos, g.p_hazard, g.logq_hazard);
+        const int64_t tw = opp_geometric(s.mt, s.pos, p_hazard, logq_hazard);
         t += tw;
         if (t < emt) {
-            const int64_t td = (int64_t)g.recovery_min + opp_geometric(mt, pos, g.p_recovery, g.logq_recovery);
-            if (n < g.cap) { w[n] = (int32_t)tw; d[n] = (int32_t)td; ++n; }
-            else gc[OPP_GEO_OVERFLOW] += 1;
+            const int64_t td = (int64_t)recovery_min + opp_geometric(s.mt, s.pos, p_recovery, logq_recovery);
+            if (n < cap) { s.wait[n] = (int32_t)tw; s.dur[n] = (int32_t)td; ++n; }
+            else s.gc[OPP_GEO_OVERFLOW] += 1;
             t += td;
         }
     }
-    gc[OPP_GEO_N] = n; gc[OPP_GEO_COUNTER] = 0; gc[OPP_GEO_FAILS] = 0;
+    s.gc[OPP_GEO_N] = n; s.gc[OPP_GEO_COUNTER] = 0;
+}
+
+// the GeometricOpponent's schedule of instance i, on its stream
+OPP_HD inline void opp_geo_sample(const OppGeoArgs &g, int i, uint32_t *mt, int32_t *pos) {
+    int32_t *gc = g.gctr + (size_t)i * OPP_GEO_CTR;
+    const OppGeoSched s{mt, pos, g.wait + (size_t)i * g.cap, g.dur + (size_t)i * g.cap, gc};
+    opp_geo_draw_schedule(s, g.emt[i], g.p_hazard, g.logq_hazard, g.p_recovery, g.logq_recovery, g.recovery_min, g.cap);
+    gc[OPP_GEO_FAILS] = 0;
+}
+
+// GeometricOpponent.attack of one opponent: its stream and schedule s, its _next_attack_time *next, OpponentSpace's previous_fails,
+// its lines [n_lines] and their weight table, the previous step's rho of the instance -> the attacked line (-1: none); *dur: its
+// duration from the schedule
+OPP_HD inline int opp_geo_attack_lines(const OppGeoSched &s, int32_t *next, bool fails, const int32_t *lines, int n_lines,
+                                       const double *weights, const float *rho, const int8_t *tv, const int32_t *line_or_pos,
+                                       const int32_t *line_ex_pos, int *dur) {
+    const int c = s.gc[OPP_GEO_COUNTER], n = s.gc[OPP_GEO_N];
+    if (c >= n) return -1;                                                             // no attack left in the schedule
+    const int32_t *w = s.wait, *d = s.dur;
+    // (int32 sums wrap as numpy's do; d[-1] of a failure before any attack is numpy's last entry)
+    if (fails) *next = (int32_t)((uint32_t)w[c] + (uint32_t)d[c > 0 ? c - 1 : n - 1]);
+    if (*next == OPP_NEXT_UNSET) *next = (int32_t)(1u + (uint32_t)w[c]);
+    *dur = d[c];
+    *next -= 1;
+    if (*next > 0) return -1;
+    s.gc[OPP_GEO_COUNTER] = c + 1;                                                     // the attack is consumed, whatever follows
+    for (int k = 0; k < n_lines; ++k) {                                                // ~status.all(): one line out -> no attack
+        const int l = lines[k];
+        if (!(tv[line_or_pos[l]] > 0 && tv[line_ex_pos[l]] > 0)) return -1;
+    }
+    if (n_lines == 1) return lines[0];
+    // Boltzmann weights on the rho ranks: rank k = lines with a lower rho, ties ranked by line order (a stable argsort)
+    double wv[OPP_MAX_ATTACK];
+    for (int k = 0; k < n_lines; ++k) {
+        const float r = rho[lines[k]];
+        int rank = 0;
+        for (int j = 0; j < n_lines; ++j) {
+            const float rj = rho[lines[j]];
+            rank += (rj < r || (rj == r && j < k)) ? 1 : 0;
+        }
+        wv[k] = weights[rank];
+    }
+    const double sum = opp_np_sum(wv, n_lines);
+    return lines[opp_choice_weighted(s.mt, s.pos, wv, n_lines, sum)];
 }
 
 // GeometricOpponent.attack for instance i -> the attacked line (-1: none); *dur: its duration from the schedule
 OPP_HD inline int opp_geo_attack(const OppArgs &o, const OppGeoArgs &g, int i, const int8_t *tv, const int32_t *line_or_pos,
                                  const int32_t *line_ex_pos, int n_line, int32_t *ctr, int32_t *gc, int *dur) {
-    const int c = gc[OPP_GEO_COUNTER], n = gc[OPP_GEO_N];
-    if (c >= n) return -1;                                                             // no attack left in the schedule
-    const int32_t *w = g.wait + (size_t)i * g.cap, *d = g.dur + (size_t)i * g.cap;
-    // (int32 sums wrap as numpy's do; d[-1] of a failure before any attack is numpy's last entry)
-    if (gc[OPP_GEO_FAILS]) ctr[OPP_CTR_NEXT] = (int32_t)((uint32_t)w[c] + (uint32_t)d[c > 0 ? c - 1 : n - 1]);
-    if (ctr[OPP_CTR_NEXT] == OPP_NEXT_UNSET) ctr[OPP_CTR_NEXT] = (int32_t)(1u + (uint32_t)w[c]);
-    *dur = d[c];
-    ctr[OPP_CTR_NEXT] -= 1;
-    if (ctr[OPP_CTR_NEXT] > 0) return -1;
-    gc[OPP_GEO_COUNTER] = c + 1;                                                       // the attack is consumed, whatever follows
-    for (int k = 0; k < o.n_attack; ++k) {                                             // ~status.all(): one line out -> no attack
-        const int l = o.lines[k];
-        if (!(tv[line_or_pos[l]] > 0 && tv[line_ex_pos[l]] > 0)) return -1;
-    }
-    if (o.n_attack == 1) return o.lines[0];
-    // Boltzmann weights on the rho ranks: rank k = lines with a lower rho, ties ranked by line order (a stable argsort)
-    const float *rho = o.rho + (size_t)i * n_line;
-    double wv[OPP_MAX_ATTACK];
-    for (int k = 0; k < o.n_attack; ++k) {
-        const float r = rho[o.lines[k]];
-        int rank = 0;
-        for (int j = 0; j < o.n_attack; ++j) {
-            const float rj = rho[o.lines[j]];
-            rank += (rj < r || (rj == r && j < k)) ? 1 : 0;
-        }
-        wv[k] = g.weights[rank];
-    }
-    const double s = opp_np_sum(wv, o.n_attack);
-    return o.lines[opp_choice_weighted(o.mt + (size_t)i * OPP_MT_N, o.mt_pos + i, wv, o.n_attack, s)];
+    const OppGeoSched s{o.mt + (size_t)i * OPP_MT_N, o.mt_pos + i, g.wait + (size_t)i * g.cap, g.dur + (size_t)i * g.cap, gc};
+    return opp_geo_attack_lines(s, &ctr[OPP_CTR_NEXT], gc[OPP_GEO_FAILS] != 0, o.lines, o.n_attack, g.weights,
+                                o.rho + (size_t)i * n_line, tv, line_or_pos, line_ex_pos, dur);
 }
 
 // OpponentSpace.attack's call of the geometric opponent with its checks: refused (and previous_fails set) when the opponent's duration
@@ -244,6 +300,82 @@ OPP_HD inline int opp_geo_asked(const OppArgs &o, const OppGeoArgs &g, int i, co
     gc[OPP_GEO_FAILS] = fails ? 1 : 0;
     if (attack >= 0) { ctr[OPP_CTR_DURATION] = duration; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
     return attack;
+}
+
+// ---- GeometricOpponentMultiArea -------------------------------------------------------------------------------------------
+OPP_HD inline OppGeoSched opp_area_sched(const OppMultiArgs &m, int i, int k) {
+    const size_t ka = (size_t)i * m.n_area + k;
+    return OppGeoSched{m.mt + ka * OPP_MT_N, m.mt_pos + ka, m.wait + ka * m.cap, m.dur + ka * m.cap, m.actr + ka * OPP_AREA_CTR};
+}
+
+// GeometricOpponentMultiArea.attack for instance i, in area order: every area's counter ticks down (clamped at -1); an area at -1 asks
+// its GeometricOpponent (with OpponentSpace's previous_fails), remembers what it returns and, for an attack, counts its duration; an
+// area still counting tells its opponent the attack continues and repeats its remembered line.  out[k]: area k's line in the
+// combined attack (-1: none) -> the number of lines in it (its cost)
+OPP_HD inline int opp_multi_attack(const OppArgs &o, const OppMultiArgs &m, int i, const int8_t *tv, const int32_t *line_or_pos,
+                                   const int32_t *line_ex_pos, int n_line, int32_t *out) {
+    const bool fails = m.fails[i] != 0;
+    const float *rho = o.rho + (size_t)i * n_line;
+    int n = 0;
+    for (int k = 0; k < m.n_area; ++k) {
+        const OppGeoSched s = opp_area_sched(m, i, k);
+        int32_t *ac = s.gc;
+        ac[OPP_AREA_CLOCK] = ac[OPP_AREA_CLOCK] > 0 ? ac[OPP_AREA_CLOCK] - 1 : -1;
+        int line;
+        if (ac[OPP_AREA_CLOCK] == -1) {
+            const int off = m.area_off[k];
+            int d = 0;
+            line = opp_geo_attack_lines(s, &ac[OPP_AREA_NEXT], fails, o.lines + off, m.area_off[k + 1] - off, m.weights + off, rho, tv,
+                                        line_or_pos, line_ex_pos, &d);
+            if (line >= 0) ac[OPP_AREA_CLOCK] = d;
+            ac[OPP_AREA_PREV] = line;
+        } else {
+            ac[OPP_AREA_NEXT] = OPP_NEXT_UNSET;                                            // tell_attack_continues
+            line = ac[OPP_AREA_PREV];
+        }
+        out[k] = line;
+        n += line >= 0 ? 1 : 0;
+    }
+    return n;
+}
+
+// OpponentSpace.attack's call of the multi-area opponent, whose duration is always 1: the combined attack is refused whole (and
+// previous_fails set) when 1 exceeds attack_max_duration or its line count exceeds the budget b.  The area counters and remembered
+// lines stay as the call left them.  -> the first line of the landed attack (-1: none); *cost: its line count
+OPP_HD inline int opp_multi_asked(const OppArgs &o, const OppMultiArgs &m, int i, const int8_t *tv, const int32_t *line_or_pos,
+                                  const int32_t *line_ex_pos, int n_line, int32_t *ctr, double b, int *cost) {
+    int32_t *out = m.attack_lines + (size_t)i * m.n_area;
+    const int n = opp_multi_attack(o, m, i, tv, line_or_pos, line_ex_pos, n_line, out);
+    bool landed = n > 0, fails = false;
+    if (1 > o.attack_duration) { landed = false; fails = true; }
+    if ((landed ? (double)n : 0.0) > b) { landed = false; fails = true; }                // duration * cost > budget
+    m.fails[i] = fails ? 1 : 0;
+    int first = -1;
+    for (int k = 0; k < m.n_area; ++k) {
+        if (!landed) out[k] = -1;
+        else if (first < 0) first = out[k];
+    }
+    if (landed) { ctr[OPP_CTR_DURATION] = 1; ctr[OPP_CTR_COOLDOWN] += o.attack_cooldown; }
+    *cost = landed ? n : 0;
+    return first;
+}
+
+// OpponentSpace.reset's GeometricOpponentMultiArea.reset for instance i: every area counter to -1, then each area's
+// GeometricOpponent.reset in area order (a new schedule from its continuing stream, _next_attack_time None); the remembered lines
+// stay
+OPP_HD inline void opp_multi_reset_instance(const OppMultiArgs &m, int i) {
+    m.fails[i] = 0;
+    for (int k = 0; k < m.n_area; ++k) m.actr[((size_t)i * m.n_area + k) * OPP_AREA_CTR + OPP_AREA_CLOCK] = -1;
+    for (int k = 0; k < m.n_area; ++k) {
+        const OppGeoSched s = opp_area_sched(m, i, k);
+        opp_geo_draw_schedule(s, m.emt[i], m.p_hazard, m.logq_hazard, m.p_recovery, m.logq_recovery, m.recovery_min, m.cap);
+        s.gc[OPP_AREA_NEXT] = OPP_NEXT_UNSET;
+    }
+}
+
+// no multi-area attack for instance i this step
+OPP_HD inline void opp_multi_none(const OppMultiArgs &m, int i) {
+    for (int k = 0; k < m.n_area; ++k) m.attack_lines[(size_t)i * m.n_area + k] = -1;
 }
 
 // ---- the opponent ---------------------------------------------------------------------------------------------------------
@@ -275,19 +407,23 @@ OPP_HD inline int opp_choose(const OppArgs &o, int i, const int8_t *tv, const in
 
 // OpponentSpace.attack for instance i (not finished, not a reset step) -> the attacked line (-1: none); *dur: its duration
 OPP_HD inline int opp_decide_instance(const OppArgs &o, int i, const int8_t *tv, const int32_t *line_or_pos, const int32_t *line_ex_pos,
-                                      int n_line, int *dur, const OppGeoArgs *g = nullptr) {
+                                      int n_line, int *dur, const OppGeoArgs *g = nullptr, const OppMultiArgs *m = nullptr) {
     int32_t *ctr = o.ctr + (size_t)i * OPP_CTR;
     double b = o.budget[i];
     const bool b64 = o.budget64[i] != 0;
     b = b64 ? b + (double)o.budget_per_ts : (double)((float)b + o.budget_per_ts);      // budget += budget_per_timestep
     ctr[OPP_CTR_DURATION] = ctr[OPP_CTR_DURATION] > 1 ? ctr[OPP_CTR_DURATION] - 1 : 0;
     ctr[OPP_CTR_COOLDOWN] = ctr[OPP_CTR_COOLDOWN] > 1 ? ctr[OPP_CTR_COOLDOWN] - 1 : 0;
-    int attack = -1;
+    int attack = -1, cost = 1;
     bool asked = false;
+    // (the multi-area opponent's duration is 1 and its attack_cooldown at most 1, so it is asked on every step: grid2op's own
+    // tell_attack_continues of it raises, and the host path refuses the configurations that would reach it)
     if (ctr[OPP_CTR_DURATION] > 0) attack = ctr[OPP_CTR_LAST];                           // the running attack continues
     else if (ctr[OPP_CTR_COOLDOWN] <= o.attack_cooldown) {
         asked = true;
-        if (o.kind == OPP_GEOMETRIC) {
+        if (o.kind == OPP_GEOMETRIC_MULTI) {
+            if (m) attack = opp_multi_asked(o, *m, i, tv, line_or_pos, line_ex_pos, n_line, ctr, b, &cost);
+        } else if (o.kind == OPP_GEOMETRIC) {
             if (g) attack = opp_geo_asked(o, *g, i, tv, line_or_pos, line_ex_pos, n_line, ctr, b);
         } else {
             attack = opp_choose(o, i, tv, line_or_pos, line_ex_pos, n_line, ctr);
@@ -298,8 +434,9 @@ OPP_HD inline int opp_decide_instance(const OppArgs &o, int i, const int8_t *tv,
     }
     if (!asked && o.kind != OPP_RANDOM_LINE) ctr[OPP_CTR_NEXT] = OPP_NEXT_UNSET;        // tell_attack_continues
     if (!asked && g) g->gctr[(size_t)i * OPP_GEO_CTR + OPP_GEO_FAILS] = 0;               // (OpponentSpace clears previous_fails)
+    if (!asked && m) { m->fails[i] = 0; opp_multi_none(*m, i); attack = -1; }
     ctr[OPP_CTR_LAST] = attack;
-    if (attack >= 0) { b = b - 1.0; o.budget64[i] = 1; }                                    // budget -= cost: float32 - int64 -> float64
+    if (attack >= 0) { b = b - (double)cost; o.budget64[i] = 1; }                           // budget -= cost: float32 - int64 -> float64
     o.budget[i] = b;
     *dur = attack >= 0 ? ctr[OPP_CTR_DURATION] : 0;
     return attack;

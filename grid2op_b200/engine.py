@@ -41,6 +41,7 @@ ABI_SYMBOLS = (
     "b200pf_env_set_state", "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats",
     "b200pf_opp_bind", "b200pf_opp_get_state", "b200pf_opp_set_state",
     "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
+    "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state",
 )
 
 
@@ -108,6 +109,21 @@ class OppGeoDesc(C.Structure):
         ("logq_recovery", C.c_double), ("recovery_min", C.c_int32), ("cap", C.c_int32), ("episode_max_time", C.c_void_p),
         ("wait", C.c_void_p), ("dur", C.c_void_p), ("gctr", C.c_void_p),
     ]
+
+
+class OppMultiDesc(C.Structure):
+    """``b200pf_opp_multi_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("n_area", C.c_int32), ("area_off", C.c_void_p), ("weights", C.c_void_p), ("p_hazard", C.c_double), ("p_recovery", C.c_double),
+        ("logq_hazard", C.c_double), ("logq_recovery", C.c_double), ("recovery_min", C.c_int32), ("cap", C.c_int32),
+        ("episode_max_time", C.c_void_p), ("mt", C.c_void_p), ("mt_pos", C.c_void_p), ("wait", C.c_void_p), ("dur", C.c_void_p),
+        ("actr", C.c_void_p), ("fails", C.c_void_p), ("attack_lines", C.c_void_p),
+    ]
+
+
+# the GeometricOpponentMultiArea's per-instance arrays in the order of b200pf_opp_multi_get_state / _set_state
+_MULTI_STATE = (("multi_mt", np.uint32), ("multi_mt_pos", np.int32), ("multi_wait", np.int32), ("multi_dur", np.int32),
+                ("multi_ctr", np.int32), ("multi_fails", np.int32))
 
 
 def make_env_desc(t: dict, state: dict):
@@ -273,9 +289,13 @@ def load_library():
     lib.b200pf_opp_geo_bind.argtypes = [vp, C.POINTER(OppGeoDesc)]
     lib.b200pf_opp_geo_get_state.argtypes = [vp, vp, vp, vp]
     lib.b200pf_opp_geo_set_state.argtypes = [vp, vp, vp, vp]
+    lib.b200pf_opp_multi_bind.argtypes = [vp, C.POINTER(OppMultiDesc)]
+    lib.b200pf_opp_multi_get_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.b200pf_opp_multi_set_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
-               "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state"):
+               "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
+               "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -787,6 +807,39 @@ class PowerFlowEngine:
     def opp_geo_set_state(self, s: dict):
         a = [np.ascontiguousarray(s[k], np.int32) for k in ("geo_wait", "geo_dur", "geo_ctr")]
         self._check(self.lib.b200pf_opp_geo_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_geo_set_state")
+
+    def opp_multi_bind(self, t: dict, d_attack_lines: int):
+        """the GeometricOpponentMultiArea's areas, constants and first state (``b200pf_opp_multi_bind``, after ``opp_bind`` with kind
+        4): ``t`` built by BatchedEnv.enable_opponent (the multi_* arrays of BatchedOpponent.get_state); ``d_attack_lines``: device
+        int32 [B, n_area] for each step's attacked lines"""
+        keep = dict(area_off=np.ascontiguousarray(t["area_off"], np.int32), weights=np.ascontiguousarray(t["weights"], np.float64),
+                    emt=np.ascontiguousarray(t["episode_max_time"], np.int32))
+        keep.update({k: np.ascontiguousarray(t[k], dt) for k, dt in _MULTI_STATE})
+        n_area, cap = int(keep["multi_wait"].shape[1]), int(keep["multi_wait"].shape[2])
+        d = OppMultiDesc(n_area=n_area, area_off=keep["area_off"].ctypes.data, weights=keep["weights"].ctypes.data,
+                         p_hazard=float(t["p_hazard"]), p_recovery=float(t["p_recovery"]), logq_hazard=float(t["logq_hazard"]),
+                         logq_recovery=float(t["logq_recovery"]), recovery_min=int(t["recovery_min"]), cap=cap,
+                         episode_max_time=keep["emt"].ctypes.data, mt=keep["multi_mt"].ctypes.data,
+                         mt_pos=keep["multi_mt_pos"].ctypes.data, wait=keep["multi_wait"].ctypes.data, dur=keep["multi_dur"].ctypes.data,
+                         actr=keep["multi_ctr"].ctypes.data, fails=keep["multi_fails"].ctypes.data, attack_lines=d_attack_lines)
+        self._check(self.lib.b200pf_opp_multi_bind(self.h, C.byref(d)), "b200pf_opp_multi_bind")
+        self._opp_multi_shape = (n_area, cap)
+        del keep
+
+    def opp_multi_get_state(self):
+        """-> dict(multi_mt uint32 [B, n_area, 624], multi_mt_pos int32 [B, n_area], multi_wait / multi_dur int32 [B, n_area, cap],
+        multi_ctr int32 [B, n_area, 6], multi_fails int32 [B]) of the GeometricOpponentMultiArea"""
+        B = self._series_batch
+        A, cap = getattr(self, "_opp_multi_shape", (0, 0))                   # (unbound: the library refuses the call)
+        shapes = dict(multi_mt=(B, A, 624), multi_mt_pos=(B, A), multi_wait=(B, A, cap), multi_dur=(B, A, cap), multi_ctr=(B, A, 6),
+                      multi_fails=(B,))
+        s = {k: np.empty(shapes[k], dt) for k, dt in _MULTI_STATE}
+        self._check(self.lib.b200pf_opp_multi_get_state(self.h, *[_ptr(s[k]) for k, _ in _MULTI_STATE]), "b200pf_opp_multi_get_state")
+        return s
+
+    def opp_multi_set_state(self, s: dict):
+        a = [np.ascontiguousarray(s[k], dt) for k, dt in _MULTI_STATE]
+        self._check(self.lib.b200pf_opp_multi_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_multi_set_state")
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")

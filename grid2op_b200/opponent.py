@@ -12,7 +12,15 @@ Restates, per instance, grid2op's ``OpponentSpace`` (grid2op/Opponent/opponentSp
   is connected (grid2op's ``~status.all()`` test), on a line drawn with Boltzmann weights ``exp(b_beta * rank)`` of the lines'
   rho ranks, for the schedule's duration.  OpponentSpace refuses it (and sets ``previous_fails``, which moves the next attack) when
   that duration exceeds ``attack_duration`` or the budget.  Ranks of equal rho follow the line order (a stable argsort): numpy's
-  default argsort is not stable for ties on every host, so that is the one place the reference's own choice can differ.
+  default argsort is not stable for ties on every host, so that is the one place the reference's own choice can differ;
+* ``GeometricOpponentMultiArea`` (geometricOpponentMultiArea.py): one GeometricOpponent per area of lines, each with its own
+  ``RandomState`` (seeded by ``randint(2**31 - 1)`` draws of the multi-area opponent's own stream, in area order), schedule and
+  ``_next_attack_time``.  Every step, each area's counter ticks down (clamped at -1); an area at -1 asks its GeometricOpponent
+  (``~status.all()``, ranks and ``b_beta`` over its own lines, OpponentSpace's shared ``previous_fails``), remembers the line and
+  counts the attack's duration, an area still counting repeats its remembered line.  The combined attack has duration 1 and costs
+  its line count; OpponentSpace refuses it whole when that exceeds the budget, and the counters stay.  With duration 1 and an
+  ``attack_cooldown`` of 0 or 1 OpponentSpace asks on every step; a larger cooldown makes it skip a step and call the multi-area
+  ``tell_attack_continues``, which raises in grid2op, so such configurations are refused here.
 
 Each instance has its own ``np.random.RandomState`` (the opponent's ``space_prng``).  The arithmetic below is numpy's own, on
 numpy scalars, as the reference does it: the budget is a float32 until the first charge (float32 - int64 promotes it to float64
@@ -29,10 +37,15 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-__all__ = ["OPPONENT_KINDS", "BatchedOpponent", "opponent_seed", "geometric_constants", "NEXT_UNSET"]
+__all__ = ["OPPONENT_KINDS", "BatchedOpponent", "opponent_seed", "geometric_constants", "NEXT_UNSET", "MAX_AREAS", "MULTI_KEYS"]
 
-OPPONENT_KINDS = {"RandomLineOpponent": 1, "WeightedRandomOpponent": 2, "GeometricOpponent": 3}
+OPPONENT_KINDS = {"RandomLineOpponent": 1, "WeightedRandomOpponent": 2, "GeometricOpponent": 3, "GeometricOpponentMultiArea": 4}
 NEXT_UNSET = -2 ** 31                  # WeightedRandomOpponent / GeometricOpponent._next_attack_time is None (device encoding)
+MAX_AREAS = 8                          # GeometricOpponentMultiArea: the device keeps fixed-size per-instance arrays
+# GeometricOpponentMultiArea's per-area counters (multi_ctr [B, n_area, 6]): schedule length, attacks consumed, _next_attack_time,
+# entries dropped at the cap, _new_attack_time_counters, _previous_attacks line (-1: None)
+AREA_N, AREA_COUNTER, AREA_NEXT, AREA_OVERFLOW, AREA_CLOCK, AREA_PREV = range(6)
+MULTI_KEYS = ("multi_mt", "multi_mt_pos", "multi_wait", "multi_dur", "multi_ctr", "multi_fails")   # its keys of get_state()
 _COST = np.int64(1)                    # BaseActionBudget of one line's set_line_status action
 _INT32_MAX = 2 ** 31 - 1
 _LOG_U_MAX = float(np.log(2.0 ** -53))  # log1p(-U) for the largest random_sample(), 1 - 2**-53: the largest geometric draw
@@ -86,11 +99,27 @@ class BatchedOpponent:
                  pmax_pmin_ratio: float = 4, delta_time_seconds: float = 300.0, episode_max_time=None):
         """``GeometricOpponent``: ``attack_every_xxx_hour``, ``average_attack_duration_hour``, ``minimum_attack_duration_hour``,
         ``pmax_pmin_ratio`` (its ``kwargs_opponent``), ``delta_time_seconds`` (the environment's step) and ``episode_max_time`` (int
-        or int [batch]: ``env.max_episode_duration()`` of each instance's scenario)."""
+        or int [batch]: ``env.max_episode_duration()`` of each instance's scenario).  ``GeometricOpponentMultiArea``: the same, with
+        ``lines`` a list of areas (lists of line ids)."""
         if kind not in OPPONENT_KINDS:
             raise ValueError(f"unknown opponent {kind!r} ({' / '.join(OPPONENT_KINDS)})")
         self.kind = kind
         self.code = OPPONENT_KINDS[kind]
+        self.multi = kind == "GeometricOpponentMultiArea"
+        if self.multi:
+            areas = [np.asarray(a, dtype=np.int64).reshape(-1) for a in lines]
+            if not 1 <= len(areas) <= MAX_AREAS:
+                raise ValueError(f"GeometricOpponentMultiArea takes 1 to {MAX_AREAS} areas")
+            if any(len(a) == 0 for a in areas):
+                raise ValueError("GeometricOpponentMultiArea: an area without lines")
+            seen = [set(a.tolist()) for a in areas]
+            if any(seen[j] & seen[k] for j in range(len(seen)) for k in range(j)):
+                raise ValueError("GeometricOpponentMultiArea: two areas share a line")
+            if int(attack_cooldown) >= 2:
+                raise ValueError("GeometricOpponentMultiArea needs attack_cooldown 0 or 1: with a longer cooldown OpponentSpace skips "
+                                 "a step and grid2op's multi-area tell_attack_continues raises")
+            self.area_off = np.concatenate([[0], np.cumsum([len(a) for a in areas])]).astype(np.int32)
+            lines = np.concatenate(areas)
         self.lines = np.asarray(lines, dtype=np.int64)
         if self.lines.ndim != 1 or not 1 <= len(self.lines) <= 64:
             raise ValueError("1 to 64 attackable lines")
@@ -123,7 +152,7 @@ class BatchedOpponent:
         self.last = np.full(batch, -1, dtype=np.int64)
         self.next_time = [None] * batch
         self.geometric = kind == "GeometricOpponent"
-        if self.geometric:
+        if self.geometric or self.multi:
             self._init_geometric(attack_every_xxx_hour, average_attack_duration_hour, minimum_attack_duration_hour, pmax_pmin_ratio,
                                  delta_time_seconds, episode_max_time)
         self.reset(np.arange(batch))
@@ -145,19 +174,43 @@ class BatchedOpponent:
             raise ValueError("episode_max_time out of range")
         self.emt = emt.astype(np.int32)
         self.pmax_pmin_ratio = pmax_pmin_ratio
-        n = len(self.lines)
-        # GeometricOpponent.attack's expressions, for every rank at once: the lines it weighs are always all attackable lines
-        self.b_beta = np.log(pmax_pmin_ratio) / (n - 1) if n > 1 else np.float64(0.0)
-        self.geo_weights = np.exp(self.b_beta * np.arange(n, dtype=np.int64))
         # every appended attack advances the schedule's time by at least recovery_min + 2 (a wait >= 1, a duration >= recovery_min + 1)
         self.cap = int(-(-int(self.emt.max()) // (self.recovery_min + 2))) + 1
+        if self.multi:
+            self._init_areas()
+            return
+        n = len(self.lines)
+        # GeometricOpponent.attack's expressions, for every rank at once: the lines it weighs are always all attackable lines
+        self.b_beta = self._b_beta(n)
+        self.geo_weights = np.exp(self.b_beta * np.arange(n, dtype=np.int64))
         self.geo_wait = np.zeros((self.batch, self.cap), dtype=np.int32)
         self.geo_dur = np.zeros((self.batch, self.cap), dtype=np.int32)
         self.geo_ctr = np.zeros((self.batch, 4), dtype=np.int32)         # schedule length, attacks consumed, previous_fails, dropped
 
-    def _geo_sample(self, i):
-        """GeometricOpponent.sample_attack_times_and_durations"""
-        rng, emt = self.rngs[i], int(self.emt[i])
+    def _b_beta(self, n):
+        return np.log(self.pmax_pmin_ratio) / (n - 1) if n > 1 else np.float64(0.0)
+
+    def _init_areas(self):
+        """GeometricOpponentMultiArea.init and seed: one GeometricOpponent per area, each seeded from the multi-area opponent's own
+        stream (``self.rngs``) in area order"""
+        A, B = len(self.area_off) - 1, self.batch
+        sizes = np.diff(self.area_off)
+        self.area_b_beta = [self._b_beta(int(n)) for n in sizes]
+        # each area's weight table at its lines' offsets (the device indexes area_off[k] + rank)
+        self.area_weights = np.concatenate([np.exp(b * np.arange(int(n), dtype=np.int64)) for b, n in zip(self.area_b_beta, sizes)])
+        max_seed = np.iinfo(np.int32).max
+        self.multi_rngs = [[np.random.RandomState(r.randint(max_seed)) for _ in range(A)] for r in self.rngs]
+        self.multi_wait = np.zeros((B, A, self.cap), dtype=np.int32)
+        self.multi_dur = np.zeros((B, A, self.cap), dtype=np.int32)
+        self.multi_ctr = np.zeros((B, A, 6), dtype=np.int32)
+        self.multi_ctr[:, :, AREA_CLOCK] = -1
+        self.multi_ctr[:, :, AREA_PREV] = -1
+        self.area_next = [[None] * A for _ in range(B)]
+        self.fails = np.zeros(B, dtype=bool)                             # OpponentSpace.previous_fails
+
+    def _geo_sample(self, rng, emt, wait, dur, ctr):
+        """GeometricOpponent.sample_attack_times_and_durations on ``rng``, into one schedule row ``wait`` / ``dur`` [cap] and its
+        counters ``ctr`` (schedule length, attacks consumed and entries dropped at the cap in words 0, 1 and 3)"""
         waits, durs = [], []
         t = 0
         while t < emt:
@@ -169,10 +222,10 @@ class BatchedOpponent:
                 durs.append(d)
                 t = t + d
         n = min(len(waits), self.cap)
-        self.geo_wait[i, :n] = np.array(waits[:n]).astype(np.int32)
-        self.geo_dur[i, :n] = np.array(durs[:n]).astype(np.int32)
-        self.geo_ctr[i, 0], self.geo_ctr[i, 1], self.geo_ctr[i, 2] = n, 0, 0
-        self.geo_ctr[i, 3] += len(waits) - n
+        wait[:n] = np.array(waits[:n]).astype(np.int32)
+        dur[:n] = np.array(durs[:n]).astype(np.int32)
+        ctr[0], ctr[1] = n, 0
+        ctr[3] += len(waits) - n
 
     # ---- OpponentSpace.reset ----------------------------------------------------------------------------------------------
     def reset(self, idx):
@@ -184,16 +237,25 @@ class BatchedOpponent:
             self.last[i] = -1
             self.next_time[i] = None
             if self.geometric:
-                self._geo_sample(int(i))
+                self._geo_sample(self.rngs[i], int(self.emt[i]), self.geo_wait[i], self.geo_dur[i], self.geo_ctr[i])
+                self.geo_ctr[i, 2] = 0                                      # previous_fails
+            if self.multi:                  # GeometricOpponentMultiArea.reset: every counter to -1, then each area's reset
+                self.fails[i] = False
+                self.multi_ctr[i, :, AREA_CLOCK] = -1
+                for k, rng in enumerate(self.multi_rngs[i]):
+                    self._geo_sample(rng, int(self.emt[i]), self.multi_wait[i, k], self.multi_dur[i, k], self.multi_ctr[i, k])
+                    self.area_next[i][k] = None
 
     # ---- OpponentSpace.attack ---------------------------------------------------------------------------------------------
     def attack(self, line_status: np.ndarray, rho: Optional[np.ndarray], live: np.ndarray):
         """One step of every live instance: ``line_status`` bool [B, n_line] and ``rho`` float32 [B, n_line] of the previous step
-        (the observation the opponent sees).  -> (attacked line int32 [B], -1 for none; attack duration int32 [B])"""
-        line = np.full(self.batch, -1, dtype=np.int32)
+        (the observation the opponent sees).  -> (attacked line int32 [B], -1 for none; attack duration int32 [B]); a
+        GeometricOpponentMultiArea gives the attacked line of every area, int32 [B, n_area] (-1: none in that area)"""
+        line = np.full((self.batch, len(self.area_off) - 1) if self.multi else self.batch, -1, dtype=np.int32)
         dur = np.zeros(self.batch, dtype=np.int32)
+        one = self._multi_attack_one if self.multi else self._attack_one
         for i in np.flatnonzero(live):
-            a, d = self._attack_one(int(i), line_status[i], None if rho is None else rho[i])
+            a, d = one(int(i), line_status[i], None if rho is None else rho[i])
             line[i], dur[i] = a, d
         return line, dur
 
@@ -236,39 +298,81 @@ class BatchedOpponent:
     def _cost(attack):
         return 0 if attack is None else _COST
 
-    def _geo_attack(self, i, status, rho):
-        """GeometricOpponent.attack"""
-        rng = self.rngs[i]
-        n, c = int(self.geo_ctr[i, 0]), int(self.geo_ctr[i, 1])
+    @staticmethod
+    def _geo_attack(rng, wait, dur, ctr, next_time, fails, lines, b_beta, status, rho):
+        """GeometricOpponent.attack of one opponent: its stream, schedule row and counters (as :meth:`_geo_sample` writes them), its
+        ``_next_attack_time``, OpponentSpace's ``previous_fails``, its lines and ``b_beta`` -> (line or None, duration or None,
+        ``_next_attack_time``)"""
+        n, c = int(ctr[0]), int(ctr[1])
         if c >= n:
-            return None, None
-        wait, dur = self.geo_wait[i, :n], self.geo_dur[i, :n]
-        if self.geo_ctr[i, 2]:
-            self.next_time[i] = wait[c] + dur[c - 1]
-        if self.next_time[i] is None:
-            self.next_time[i] = 1 + wait[c]
+            return None, None, next_time
+        wait, dur = wait[:n], dur[:n]
+        if fails:
+            next_time = wait[c] + dur[c - 1]
+        if next_time is None:
+            next_time = 1 + wait[c]
         attack_duration = dur[c]
-        self.next_time[i] -= 1
-        if self.next_time[i] > 0:
-            return None, None
-        self.geo_ctr[i, 1] = c + 1
-        st = np.asarray(status, dtype=bool)[self.lines]
+        next_time -= 1
+        if next_time > 0:
+            return None, None, next_time
+        ctr[1] = c + 1
+        st = np.asarray(status, dtype=bool)[lines]
         if ~st.all():
-            return None, None
-        if len(self.lines) == 1:
-            return int(self.lines[0]), attack_duration
-        r = np.asarray(rho, dtype=np.float32)[self.lines]
+            return None, None, next_time
+        if len(lines) == 1:
+            return int(lines[0]), attack_duration, next_time
+        r = np.asarray(rho, dtype=np.float32)[lines]
         temp = r.argsort(kind="stable")
         rho_ranks = np.empty_like(temp)
         rho_ranks[temp] = np.arange(len(r))
-        raw_probabilities = np.exp(self.b_beta * rho_ranks)
+        raw_probabilities = np.exp(b_beta * rho_ranks)
         b_probabilities = raw_probabilities / raw_probabilities.sum()
-        return int(rng.choice(self.lines, p=b_probabilities)), attack_duration
+        return int(rng.choice(lines, p=b_probabilities)), attack_duration, next_time
+
+    def _multi_attack_one(self, i, status, rho):
+        """OpponentSpace.attack with GeometricOpponentMultiArea.attack -> (line int32 [n_area], -1 where none; duration)"""
+        self.budget[i] = self.budget[i] + self.budget_per_ts
+        self.duration[i] = max(0, self.duration[i] - 1)
+        self.cooldown[i] = max(0, self.cooldown[i] - 1)
+        if self.duration[i] > 0 or self.cooldown[i] > self.attack_cooldown:     # (attack_cooldown <= 1 and duration 1: never)
+            raise RuntimeError("OpponentSpace skipped the GeometricOpponentMultiArea, whose tell_attack_continues raises")
+        ctr = self.multi_ctr[i]
+        ctr[:, AREA_CLOCK] -= 1
+        ctr[ctr[:, AREA_CLOCK] < -1, AREA_CLOCK] = -1
+        fails = self.fails[i]
+        for k in range(len(ctr)):
+            if ctr[k, AREA_CLOCK] == -1:
+                lines = self.lines[self.area_off[k]:self.area_off[k + 1]]
+                a, d, self.area_next[i][k] = self._geo_attack(self.multi_rngs[i][k], self.multi_wait[i, k], self.multi_dur[i, k], ctr[k],
+                                                              self.area_next[i][k], fails, lines, self.area_b_beta[k], status, rho)
+                if a is not None:
+                    ctr[k, AREA_CLOCK] = d
+                ctr[k, AREA_PREV] = -1 if a is None else a
+            else:
+                self.area_next[i][k] = None                                 # tell_attack_continues
+        out = ctr[:, AREA_PREV].astype(np.int32)                            # the combined attack: every area's remembered line
+        n = int((out >= 0).sum())
+        attack, duration, fails = n > 0, 1, False
+        if duration > self.attack_duration:
+            attack, fails = False, True
+        if duration * (np.int64(n) if attack else 0) > self.budget[i]:
+            attack, fails = False, True
+        self.fails[i] = fails
+        if attack:
+            self.duration[i] = duration
+            self.cooldown[i] += self.attack_cooldown
+        else:
+            out[:] = -1
+        self.budget[i] = self.budget[i] - (np.int64(n) if attack else 0)
+        self.last[i] = out[out >= 0][0] if attack else -1
+        return out, (int(self.duration[i]) if attack else 0)
 
     def _opponent_attack(self, i, status, rho):
         rng = self.rngs[i]
         if self.geometric:
-            return self._geo_attack(i, status, rho)
+            a, d, self.next_time[i] = self._geo_attack(rng, self.geo_wait[i], self.geo_dur[i], self.geo_ctr[i], self.next_time[i],
+                                                       self.geo_ctr[i, 2], self.lines, self.b_beta, status, rho)
+            return a, d
         if self.weighted:
             if self.next_time[i] is None:
                 self.next_time[i] = 1 + rng.randint(self.attack_period)
@@ -291,7 +395,11 @@ class BatchedOpponent:
     def get_state(self):
         """-> dict(budget float64 [B], budget64 uint8 [B], ctr int32 [B, 4], mt uint32 [B, 624], mt_pos int32 [B]); a
         GeometricOpponent adds geo_wait / geo_dur int32 [B, cap] (the schedules) and geo_ctr int32 [B, 4] (schedule length, attacks
-        consumed, previous_fails, schedule entries dropped at the cap)"""
+        consumed, previous_fails, schedule entries dropped at the cap); a GeometricOpponentMultiArea adds its areas' streams
+        multi_mt uint32 [B, n_area, 624] / multi_mt_pos int32 [B, n_area], their schedules multi_wait / multi_dur int32
+        [B, n_area, cap], their counters multi_ctr int32 [B, n_area, 6] (schedule length, attacks consumed, _next_attack_time,
+        entries dropped at the cap, _new_attack_time_counters, _previous_attacks line) and multi_fails int32 [B] (previous_fails);
+        its mt / mt_pos are the multi-area opponent's own stream, which only seeded the areas"""
         B = self.batch
         ctr = np.empty((B, 4), dtype=np.int32)
         ctr[:, 0], ctr[:, 1], ctr[:, 2] = self.duration, self.cooldown, self.last
@@ -305,6 +413,18 @@ class BatchedOpponent:
                  budget64=np.array([b.dtype == np.float64 for b in self.budget], dtype=np.uint8), ctr=ctr, mt=mt, mt_pos=pos)
         if self.geometric:
             s.update(geo_wait=self.geo_wait.copy(), geo_dur=self.geo_dur.copy(), geo_ctr=self.geo_ctr.copy())
+        if self.multi:
+            A = len(self.area_off) - 1
+            amt = np.empty((B, A, 624), dtype=np.uint32)
+            apos = np.empty((B, A), dtype=np.int32)
+            for i in range(B):
+                for k, r in enumerate(self.multi_rngs[i]):
+                    st = r.get_state()
+                    amt[i, k], apos[i, k] = st[1], st[2]
+            actr = self.multi_ctr.copy()
+            actr[:, :, AREA_NEXT] = [[NEXT_UNSET if t is None else int(t) for t in row] for row in self.area_next]
+            s.update(multi_mt=amt, multi_mt_pos=apos, multi_wait=self.multi_wait.copy(), multi_dur=self.multi_dur.copy(),
+                     multi_ctr=actr, multi_fails=self.fails.astype(np.int32))
         return s
 
     def set_state(self, s):
@@ -317,3 +437,10 @@ class BatchedOpponent:
             self.geo_wait[:], self.geo_dur[:], self.geo_ctr[:] = s["geo_wait"], s["geo_dur"], s["geo_ctr"]
         else:
             self.next_time = [None if int(t) == NEXT_UNSET else int(t) for t in s["ctr"][:, 3]]
+        if self.multi:
+            for i in range(self.batch):
+                for k, r in enumerate(self.multi_rngs[i]):
+                    r.set_state(("MT19937", np.asarray(s["multi_mt"][i, k], dtype=np.uint32), int(s["multi_mt_pos"][i, k]), 0, 0.0))
+            self.multi_wait[:], self.multi_dur[:], self.multi_ctr[:] = s["multi_wait"], s["multi_dur"], s["multi_ctr"]
+            self.area_next = [[None if int(t) == NEXT_UNSET else np.int32(t) for t in row] for row in s["multi_ctr"][:, :, AREA_NEXT]]
+            self.fails[:] = np.asarray(s["multi_fails"]) != 0

@@ -404,7 +404,8 @@ int b200pf_env_stats(const b200pf_handle *h, int64_t *out8);
  * duration, current attack cooldown, last attacked line or -1, steps to the weighted opponent's next attack or INT32_MIN for
  * none), mt uint32 [batch][624] and mt_pos int32 [batch].  Unbound (b200pf_opp_bind never called), nothing of the above runs. */
 typedef struct b200pf_opp_desc {
-    int32_t kind;                       /* 1: RandomLineOpponent, 2: WeightedRandomOpponent, 3: GeometricOpponent */
+    int32_t kind;                       /* 1: RandomLineOpponent, 2: WeightedRandomOpponent, 3: GeometricOpponent,
+                                           4: GeometricOpponentMultiArea */
     int32_t n_attack;                   /* attackable lines, 1..64 */
     const int32_t *lines;               /* [n_attack] their line ids */
     const double *rho_norm;             /* [n_attack] rho normalisation (kind 2) */
@@ -442,6 +443,37 @@ typedef struct b200pf_opp_geo_desc {
 int b200pf_opp_geo_bind(b200pf_handle *h, const b200pf_opp_geo_desc *desc);
 int b200pf_opp_geo_get_state(b200pf_handle *h, int32_t *wait, int32_t *dur, int32_t *gctr);
 int b200pf_opp_geo_set_state(b200pf_handle *h, const int32_t *wait, const int32_t *dur, const int32_t *gctr);
+
+/* GeometricOpponentMultiArea (kind 4): b200pf_opp_bind with kind 4 and the lines of every area one after the other (rho_norm and
+ * attack_period unused; mt is the multi-area opponent's own stream, which only seeds the areas and is not drawn from again), then
+ * b200pf_opp_multi_bind; b200pf_env_step and b200pf_env_reset refuse a kind-4 opponent without it.  Each area is a GeometricOpponent
+ * with its own stream (mt uint32 [batch][n_area][624], mt_pos int32 [batch][n_area]), its own schedule (wait / dur int32
+ * [batch][n_area][cap]) and six int32 counters (actr [batch][n_area][6]: schedule length, attacks consumed, _next_attack_time or
+ * INT32_MIN for None, schedule entries dropped at the cap, _new_attack_time_counters, _previous_attacks line or -1); fails int32
+ * [batch] is OpponentSpace's previous_fails.  Every step asks every live instance (the opponent's duration is always 1); the
+ * combined attack costs one per line and is refused whole.  attack_lines (device, caller-owned, int32 [batch][n_area]) receives
+ * each step's attacked line per area (-1: none); b200pf_opp_bind's attack_line receives the first of them (-1: none) and attack_dur
+ * 1 or 0.  b200pf_env_reset draws every reset instance's area schedules on the device, in area order. */
+typedef struct b200pf_opp_multi_desc {
+    int32_t n_area;                     /* 1..8 */
+    const int32_t *area_off;            /* [n_area + 1] area k's lines are lines[area_off[k] .. area_off[k + 1]), none empty */
+    const double *weights;              /* [n_attack] area k's np.exp(b_beta_k * r) at area_off[k] + r */
+    double p_hazard, p_recovery;        /* attack hazard rate, recovery rate */
+    double logq_hazard, logq_recovery;  /* log(1 - p) of both */
+    int32_t recovery_min;               /* minimum attack duration in steps */
+    int32_t cap;                        /* schedule entries per instance and area, >= 1 */
+    const int32_t *episode_max_time;    /* [batch] */
+    const uint32_t *mt;                 /* [batch][n_area][624] the areas' initial streams */
+    const int32_t *mt_pos;              /* [batch][n_area] */
+    const int32_t *wait, *dur;          /* [batch][n_area][cap] the initial schedules */
+    const int32_t *actr;                /* [batch][n_area][6] their counters */
+    const int32_t *fails;               /* [batch] previous_fails */
+    int32_t *attack_lines;              /* device [batch][n_area] per-step output */
+} b200pf_opp_multi_desc;
+int b200pf_opp_multi_bind(b200pf_handle *h, const b200pf_opp_multi_desc *desc);
+int b200pf_opp_multi_get_state(b200pf_handle *h, uint32_t *mt, int32_t *mt_pos, int32_t *wait, int32_t *dur, int32_t *actr, int32_t *fails);
+int b200pf_opp_multi_set_state(b200pf_handle *h, const uint32_t *mt, const int32_t *mt_pos, const int32_t *wait, const int32_t *dur,
+                               const int32_t *actr, const int32_t *fails);
 
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */

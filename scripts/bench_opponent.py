@@ -2,7 +2,8 @@
 of scripts/bench_env_tensor.py: random one-substation and one-line actions drawn on the GPU with a seeded torch generator, then
 observe, finished instances reset on the device; protections off and on; case14 at batch 4096 (RandomLineOpponent on the lines of
 rte_case14_opponent), l2rpn_neurips_2020_track1 at batch 1024 (its WeightedRandomOpponent) and l2rpn_wcci_2022_dev at batch 1024
-(its GeometricOpponent, with the environment's own constants: its device resets draw a new attack schedule).  The first two use their
+(its GeometricOpponent, with the environment's own constants: its device resets draw a new attack schedule) and l2rpn_idf_2023 at
+batch 1024 (its GeometricOpponentMultiArea, three areas, with its own constants).  The first two use their
 environments' constants with a small initial budget, so that attacks run from the first steps on.  A host clock around K steps that end in a device
 synchronise, after warm-up.  Prints env.step/s (min / median / max over the repeats), the extra bytes per step the opponent moves, and
 the card and its power limit read in the same run.
@@ -37,6 +38,14 @@ OPPONENTS = {
                                        "102_104_61"],
                                 attack_duration=96, attack_cooldown=12, budget_per_ts=0.17, init_budget=144.0, attack_every_xxx_hour=24,
                                 average_attack_duration_hour=4, minimum_attack_duration_hour=1),
+    # the environment's own GeometricOpponentMultiArea (config.py): three areas, attacks every 32 h on average, 2 h long, at least 1 h
+    "l2rpn_idf_2023": dict(kind="GeometricOpponentMultiArea",
+                           lines=[["26_31_106", "21_22_93", "17_18_88", "4_10_162", "12_14_68", "29_37_117"],
+                                  ["62_58_180", "62_63_160", "48_50_136", "48_53_141", "41_48_131", "39_41_121", "43_44_125", "44_45_126",
+                                   "34_35_110", "54_58_154"],
+                                  ["74_117_81", "93_95_43", "88_91_33", "91_92_37", "99_105_62", "102_104_61"]],
+                           attack_duration=96, attack_cooldown=0, budget_per_ts=0.51, init_budget=1000.0, attack_every_xxx_hour=32,
+                           average_attack_duration_hour=2, minimum_attack_duration_hour=1),
 }
 
 
@@ -76,7 +85,7 @@ def run(name, B, protections, steps, warmup, repeats):
         e.observe()
         e.reset_instances(done.clone())
         if count and "opponent_attack_line" in info:
-            attacks[mode] += int((info["opponent_attack_line"] >= 0).sum())
+            attacks[mode] += int((info["opponent_attack_line"] >= 0).reshape(B, -1).any(1).sum())
 
     def timed(mode):
         for _ in range(warmup):
@@ -112,9 +121,13 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--only", default=None, help="one workload (environment name)")
     args = ap.parse_args()
     print("card, power limit:", card())
-    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024), ("l2rpn_wcci_2022_dev", 1024)):
+    for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024), ("l2rpn_wcci_2022_dev", 1024),
+                    ("l2rpn_idf_2023", 1024)):
+        if args.only and name != args.only:
+            continue
         for prot in (False, True):
             run(name, B, prot, args.steps, args.warmup, args.repeats)
 
