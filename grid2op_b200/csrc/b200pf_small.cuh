@@ -373,7 +373,8 @@ __device__ void solve_small(const DevGrid &g, const RunArgs &a, const SmallLayou
                 if (colth >= 0 && cj >= 0) Mr[cj] -= b;                 // reference angle is 0 (pPB:473)
                 rhs -= side ? -g.line_pshift[l] : g.line_pshift[l];
             }
-            if (colth >= 0) { Mr[colth] = dsum; Mr[n1] = rhs; }
+            // (+=: a line with both ends on this bus took b twice off the diagonal above, which cancels its 2 b in dsum)
+            if (colth >= 0) { Mr[colth] += dsum; Mr[n1] = rhs; }
         }
         __syncwarp();
         if (!gj_small_d(Md, n1, pitch, xd, lane)) { small_fail(g, a, inst, ST_DIV, 0, lane); return; }
@@ -402,7 +403,7 @@ __device__ void solve_small(const DevGrid &g, const RunArgs &a, const SmallLayou
                 const float ps = (float)g.line_pshift[l];
                 rhs -= side ? -ps : ps;
             }
-            if (colth >= 0) { Mr[colth] = dsum; Mr[n1] = rhs; }
+            if (colth >= 0) { Mr[colth] += dsum; Mr[n1] = rhs; }            // (+=: as in the DC system)
         }
         __syncwarp();
         if (!gj_small_f(J, n1, pitch, xs, lane)) { small_fail(g, a, inst, ST_DIV, 0, lane); return; }
