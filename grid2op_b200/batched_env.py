@@ -113,6 +113,7 @@ class BatchedEnv(BatchedDoNothing):
         self._dev = None
         self._authority = "host"
         self._opp = None                                                   # line-attack opponent (:meth:`enable_opponent`)
+        self._alerts = None                                                # line alerts (:meth:`enable_alerts`)
 
     # ------------------------------------------------------------------------------------------------------------
     def _bus_cap(self) -> int:
@@ -267,11 +268,18 @@ class BatchedEnv(BatchedDoNothing):
                 self._topo_dirty = True
                 self._cap_dirty[ii[was_on]] = True
 
-    def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False):
+    def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None):
         """One env.step of every instance.  ``sub_id`` int [B] (-1: none) with ``sub_bus`` int8 [B, >= max_sub_size] (busbar per
         element of that substation in topology-vector order, 0 = leave); ``line_id`` int [B] (-1: none) with ``line_status``
-        int [B] (+1 reconnect / -1 disconnect).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the
-        device (:meth:`fetch`)."""
+        int [B] (+1 reconnect / -1 disconnect); ``raise_alert`` bool [B, dim_alerts] (:meth:`enable_alerts`; None: no alert,
+        ignored on a reset step).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the device (:meth:`fetch`)."""
+        if raise_alert is not None:
+            if self._alerts is None:
+                raise ValueError("raise_alert without enable_alerts()")
+            raise_alert = np.asarray(raise_alert)
+            if raise_alert.shape != (self.batch, self._alerts.n) or raise_alert.dtype.kind not in "bui":
+                raise ValueError(f"raise_alert must be a bool array of shape {(self.batch, self._alerts.n)}")
+            raise_alert = raise_alert != 0
         self._to_host()
         gm = self.gm
         opp = None
@@ -328,6 +336,10 @@ class BatchedEnv(BatchedDoNothing):
                 sc[(sc > 0) & live[:, None]] -= 1
                 sc[aff_s] = self.cd_sub
         newly_done = live & (status != 0)
+        alert_reward = None
+        if self._alerts is not None:          # after the attack; an instance finished before the step keeps its alert state
+            alert_reward = self._alerts.step(None if from_reset else raise_alert, opp[0] if opp is not None else None,
+                                             live & (not from_reset), newly_done).copy()
         self.done |= newly_done
         self.row = self.row + 1
         self.n_steps += 1
@@ -341,7 +353,62 @@ class BatchedEnv(BatchedDoNothing):
         info = {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done, "is_illegal": self.is_illegal.copy()}
         if opp is not None:
             info["opponent_attack_line"], info["opponent_attack_duration"] = opp
+        if alert_reward is not None and self._alerts.reward:
+            info["rewards"] = {"alert": alert_reward}
         return rho, self.done.copy(), info
+
+    # ---- line alerts ------------------------------------------------------------------------------------------------------
+    def enable_alerts(self, alertable_lines, *, alert_time_window: int = 12, reward: bool = True, reward_min_no_blackout: float = -1.0,
+                      reward_min_blackout: float = -10.0, reward_max_no_blackout: float = 1.0, reward_max_blackout: float = 2.0,
+                      reward_end_episode_bonus: float = 1.0):
+        """grid2op's line alerts (l2rpn_idf_2023) for every instance: ``alertable_lines``, names (``GridModel.name_line``) or ids
+        in grid2op's order (a list of areas, as the config's ``lines_attacked``, is flattened), at most 64; ``alert_time_window``:
+        the ``ALERT_TIME_WINDOW`` parameter; ``reward``: compute ``AlertReward`` with these constants into
+        ``info["rewards"]["alert"]`` (float64 [B], 0 for an instance finished before the step) and ``was_alert_used_after_attack``.
+        The attacked lines are those of the opponent :meth:`enable_opponent` binds (none without one).  From then on :meth:`step`
+        / :meth:`step_tensors` take ``raise_alert``, and :meth:`observe` fills the seven alert attributes.  Call it before
+        :meth:`enable_observation` (the vector's width depends on ``dim_alerts``).  ``reward_end_episode_bonus`` is kept but never
+        paid: this environment has no end of chronics, the caller resets."""
+        from .alert import BatchedAlerts
+        if self._obs is not None:
+            raise RuntimeError("enable_alerts() before enable_observation(): the observation width depends on dim_alerts")
+        names = list(getattr(self.gm, "name_line", []))
+        flat = []
+        for x in alertable_lines:
+            flat.extend(x if isinstance(x, (list, tuple)) else [x])
+        if len(flat) > 64:
+            raise ValueError("more than 64 alertable lines")
+        ids = []
+        for x in flat:
+            if isinstance(x, str):
+                if x not in names:
+                    raise ValueError(f"unknown line {x!r}")
+                ids.append(names.index(x))
+            else:
+                ids.append(int(x))
+        if not ids or any(not 0 <= l < self.gm.n_line for l in ids):
+            raise ValueError("alertable line out of range (or no line)")
+        if len(set(ids)) != len(ids):
+            raise ValueError("alertable line listed twice")
+        if int(alert_time_window) <= 0:
+            raise ValueError("alert_time_window must be >= 1")
+        self._to_host()
+        self._alerts = BatchedAlerts(ids, self.batch, window=int(alert_time_window), reward=reward,
+                                     reward_min_no_blackout=reward_min_no_blackout, reward_min_blackout=reward_min_blackout,
+                                     reward_max_no_blackout=reward_max_no_blackout, reward_max_blackout=reward_max_blackout,
+                                     reward_end_episode_bonus=reward_end_episode_bonus)
+        if self._dev is not None:
+            self._alert_bind_device()
+        return self._alerts.n
+
+    def alert_state(self) -> dict:
+        """the alert state of every instance as the device keeps it (:data:`grid2op_b200.alert.ALERT_STATE`): last_alert, already
+        (_is_already_attacked) uint8 [B, n]; tsl_alert, duration, tsl_attack, under_alert, was_used int32 [B, n]; total int32
+        [B]; AlertReward's ts_attack / launched uint8 [B, window + 2, n], current uint8 [B, n] and cur_id int32 [B]"""
+        if self._alerts is None:
+            raise RuntimeError("call enable_alerts() first")
+        self._to_host()
+        return self._alerts.get_state()
 
     # ---- line-attack opponent ---------------------------------------------------------------------------------------------
     def enable_opponent(self, kind: str, lines_attacked, *, attack_duration: int, attack_cooldown: int, budget_per_ts: float,
@@ -489,6 +556,8 @@ class BatchedEnv(BatchedDoNothing):
         self.row[idx] = rows
         if self._opp is not None:
             self._opp.reset(idx)
+        if self._alerts is not None:
+            self._alerts.reset(idx)
         self.engine.series_reset_instances(idx, t_new=rows % self.chron.shape[1], topo_rows=self.topo[idx])
         self._cap_dirty[idx] = True
         if self.tight_cap:
@@ -507,7 +576,8 @@ class BatchedEnv(BatchedDoNothing):
         if reward not in ob.REWARDS:
             raise ValueError(f"unknown reward class {reward!r} (RedispReward, L2RPNReward or None)")
         gm = self.gm
-        seg, n_obs = ob.obs_spec(gm, attrs)
+        n_alert = self._alerts.n if self._alerts is not None else 0
+        seg, n_obs = ob.obs_spec(gm, attrs, n_alert)
         folders = list(scenarios) if scenarios is not None else list_scenarios(os.path.join(env_dir, "chronics"))
         if len(folders) != self.chron.shape[0]:
             raise ValueError(f"{len(folders)} scenario folders for {self.chron.shape[0]} scenarios of the chronics array")
@@ -520,17 +590,18 @@ class BatchedEnv(BatchedDoNothing):
                  maint_time=self._maint_time, maint_dur=self._maint_dur, reward_kind=ob.REWARDS[reward],
                  reward=ob.reward_constants(gen, dt_min) if gen["available"] else dict(max_regret=0.0, reward_min=0.0, reward_illegal=0.0,
                                                                                        dts_hours=dt_min / 60.0),
-                 soft_thr=self.soft_overflow_threshold)
+                 soft_thr=self.soft_overflow_threshold, n_alert=n_alert)
         if reward == "L2RPNReward":
             t["reward"]["reward_min"] = 0.0
         self.engine.obs_bind(t)
         self._obs = dict(tables=t, n_obs=n_obs, reward=reward, reset=np.ones(self.batch, dtype=bool),
-                         host_in=np.zeros((self.batch, gm.n_line + gm.n_sub + 3), dtype=np.int32))
+                         host_in=np.zeros((self.batch, gm.n_line + gm.n_sub + 3 + (6 * n_alert + 1 if n_alert else 0)), dtype=np.int32))
         return n_obs
 
     def observe_inputs(self) -> np.ndarray:
         """int32 [B, n_line + n_sub + 3]: the per-instance values only the host knows (cooldowns, current_step, step stamp, flags
-        illegal / game over / reset) — what one observe launch copies to the device."""
+        illegal / game over / reset) — what one observe launch copies to the device; with alerts, 6 dim_alerts + 1 more columns
+        (the alert values, :meth:`grid2op_b200.alert.BatchedAlerts.obs_record`)."""
         self._to_host()
         gm, o = self.gm, self._obs
         h = o["host_in"]
@@ -538,6 +609,8 @@ class BatchedEnv(BatchedDoNothing):
         h[:, :nl] = self.line_cooldown; h[:, nl:nl + ns] = self.sub_cooldown
         h[:, nl + ns] = self.current_step; h[:, nl + ns + 1] = self.n_steps
         h[:, nl + ns + 2] = self.is_illegal * 1 + self.done * 2 + o["reset"] * 4
+        if self._alerts is not None:
+            h[:, nl + ns + 3:] = self._alerts.obs_record()
         return h
 
     def observe(self, obs_out=None, reward_out=None):
@@ -623,6 +696,8 @@ class BatchedEnv(BatchedDoNothing):
         self._illegal_seen = 0
         if self._opp is not None:
             self._opp_bind_device()
+        if self._alerts is not None:
+            self._alert_bind_device()
         return st
 
     def _opp_bind_device(self):
@@ -650,6 +725,15 @@ class BatchedEnv(BatchedDoNothing):
                                        d["opp_lines"].data_ptr())
         self._authority = "host"              # (the next step_tensors pushes the whole state, the opponent's included)
 
+    def _alert_bind_device(self):
+        """the alert constants to the device; the step's raise_alert and AlertReward are device buffers of ours"""
+        import torch
+        d, a, B = self._dev, self._alerts, self.batch
+        d["alert_raise"] = torch.zeros((B, a.n), dtype=torch.uint8, device=d["device"])
+        d["alert_reward"] = torch.zeros(B, dtype=torch.float64, device=d["device"])
+        self.engine.alert_bind(a, d["alert_raise"].data_ptr(), d["alert_reward"].data_ptr())
+        self._authority = "host"              # (the next step_tensors pushes the whole state, the alerts' included)
+
     def _to_device(self):
         """hand the host state to the tensor path"""
         import torch
@@ -670,6 +754,8 @@ class BatchedEnv(BatchedDoNothing):
                 self.engine.opp_geo_set_state(s)
             if self._opp.multi:
                 self.engine.opp_multi_set_state(s)
+        if self._alerts is not None:
+            self.engine.alert_set_state(self._alerts.get_state())
         self._illegal_seen = self.engine.env_stats()["n_illegal"]
         self._authority = "device"
 
@@ -695,10 +781,13 @@ class BatchedEnv(BatchedDoNothing):
             if self._opp.multi:
                 s.update(self.engine.opp_multi_get_state())
             self._opp.set_state(s)
+        if self._alerts is not None:
+            self._alerts.set_state(self.engine.alert_get_state())
+            self._alerts.reward_out[:] = self._dev["alert_reward"].cpu().numpy()
         if self.tight_cap and self._cap_dirty.any():
             self.nb_cap = self._bus_cap()
 
-    def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False):
+    def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None):
         """:meth:`step` with the actions as CUDA tensors and the state kept on the device: ``sub_id`` int32 / int64 [B] (-1: none)
         with ``sub_bus`` int8 / int32 / int64 [B, >= max_sub_size]; ``line_id`` int32 / int64 [B] (-1: none) with ``line_status``
         int32 / int64 [B] (> 0 reconnect / < 0 disconnect).  Same semantics and bit-identical state as :meth:`step`; ordered against torch's current
@@ -706,7 +795,8 @@ class BatchedEnv(BatchedDoNothing):
         override), ``iters``, ``newly_done``, ``is_illegal``, ``disc_lines`` (protections on, else None).  The returned tensors
         are the environment's own buffers: the next step overwrites them.  The host waits once per step for a few words (and
         copies back the changed topology rows when the plans have to be looked up, which waits again).  An id or busbar out of
-        range raises ValueError and changes nothing."""
+        range raises ValueError and changes nothing.  ``raise_alert``: bool / uint8 CUDA tensor [B, dim_alerts] (:meth:`enable_alerts`;
+        None: no alert); ``info["rewards"]["alert"]`` is then the environment's float64 [B] buffer of the AlertReward."""
         import torch
         d = self._tensor_state()
         dev, B = d["device"], self.batch
@@ -737,8 +827,17 @@ class BatchedEnv(BatchedDoNothing):
         if line_id is not None:
             lid = ids(line_id, "line_id")
             lst = ids(line_status, "line_status")
+        if raise_alert is not None:
+            if self._alerts is None:
+                raise ValueError("raise_alert without enable_alerts()")
+            _check_tensor(raise_alert, "raise_alert", (B, self._alerts.n), (torch.bool, torch.uint8), dev)
         if self._authority != "device":
             self._to_device()
+        if self._alerts is not None:                      # (on torch's stream: ordered before the engine's launches below)
+            if raise_alert is None:
+                d["alert_raise"].zero_()
+            else:
+                d["alert_raise"].copy_(raise_alert != 0)
         cur, eng = self._streams()
         eng.wait_stream(cur)
         try:
@@ -761,6 +860,8 @@ class BatchedEnv(BatchedDoNothing):
         if self._opp is not None:
             info["opponent_attack_line"] = d["opp_lines"] if self._opp.multi else d["opp_line"]
             info["opponent_attack_duration"] = d["opp_dur"]
+        if self._alerts is not None and self._alerts.reward:
+            info["rewards"] = {"alert": d["alert_reward"]}
         return d["rho"], d["done"], info
 
     def _reset_tensors(self, mask, rows=None):

@@ -126,6 +126,9 @@ struct b200pf_handle {
     std::vector<void *> opp_allocs;
     OppGeoArgs opp_geo{}; bool opp_geo_bound = false;            // kind OPP_GEOMETRIC (b200pf_opp_geo_bind; its buffers in opp_allocs)
     OppMultiArgs opp_multi{}; bool opp_multi_bound = false;      // kind OPP_GEOMETRIC_MULTI (b200pf_opp_multi_bind; likewise)
+    // line alerts of the device environment (b200pf_alert_bind)
+    AlertArgs alert{}; int alert_batch = 0;
+    std::vector<void *> alert_allocs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -337,6 +340,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     for (void *p : h->env_allocs) cudaFree(p);
     if (h->h_env_ctl) cudaFreeHost(h->h_env_ctl);
     for (void *p : h->opp_allocs) cudaFree(p);
+    for (void *p : h->alert_allocs) cudaFree(p);
     delete h;
     return 0;
 }
@@ -1737,6 +1741,7 @@ extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
         return fail(B200PF_E_ARG, "generator tables missing");
     if (g.n_sto && (!d->sto_charge0 || !d->sto_loss_step)) return fail(B200PF_E_ARG, "storage tables missing");
     if (d->reward_kind < B200PF_REWARD_NONE || d->reward_kind > B200PF_REWARD_L2RPN) return fail(B200PF_E_ARG, "unknown reward kind");
+    if (d->n_alert < 0 || d->n_alert > ALERT_MAX_LINES) return fail(B200PF_E_ARG, "n_alert out of range");
     for (int s = 0; s < d->n_seg; ++s)
         if (d->seg[3 * s] < 0 || d->seg[3 * s] >= OS_N_SOURCES || d->seg[3 * s + 1] < 0 || d->seg[3 * s + 2] < 0 ||
             d->seg[3 * s + 1] + d->seg[3 * s + 2] > d->n_obs) return fail(B200PF_E_ARG, "observation segment out of range");
@@ -1782,7 +1787,8 @@ extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
     a.n_seg = d->n_seg; a.n_obs = d->n_obs; a.delta_time = d->delta_time; a.redisp_available = d->redisp_available;
     a.reward_kind = d->reward_kind; a.max_regret = d->max_regret; a.reward_min = d->reward_min; a.reward_illegal = d->reward_illegal;
     a.dts_hours = d->dts_hours; a.soft_thr = d->soft_thr;
-    a.host_stride = g.n_line + g.n_sub + 3;
+    a.n_alert = d->n_alert;
+    a.host_stride = g.n_line + g.n_sub + 3 + (d->n_alert ? 6 * d->n_alert + 1 : 0);
     if (cudaMallocHost(&h->h_obs_in, B * a.host_stride * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
     void *din = nullptr;
     if ((rc = zeros(B * a.host_stride * 4, 0, &din))) return rc;
@@ -1946,6 +1952,29 @@ extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
 static inline unsigned env_grid(int n) { return (unsigned)((n + 127) / 128); }
 
 // the opponent the env launches run: the bound one, or none (kind OPP_NONE)
+static OppArgs env_opp(const b200pf_handle *h);
+
+// the line alerts the env launches run (n = 0: none), reading the attacked lines the opponent of the same launches writes
+static AlertArgs env_alert(const b200pf_handle *h) {
+    if (!h->alert_batch || h->alert_batch != h->env_batch) return AlertArgs{};
+    AlertArgs al = h->alert;
+    const OppArgs o = env_opp(h);
+    if (o.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound) { al.attack = h->opp_multi.attack_lines; al.attack_stride = h->opp_multi.n_area; }
+    else if (o.kind != OPP_NONE) { al.attack = o.attack_line; al.attack_stride = 1; }
+    return al;
+}
+
+// the observe input record the env launches write: NULL when the observation layer is not bound to this series; an error
+// when its alert values do not match the bound alerts
+static int env_obs_record(const b200pf_handle *h, const AlertArgs &al, int32_t **rec, int *stride) {
+    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
+    *rec = obs ? h->d_obs_in : nullptr;
+    *stride = obs ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3;
+    if (obs && h->obs.n_alert != al.n)
+        return fail(B200PF_E_STATE, "the observation layer and the line alerts disagree on dim_alerts (b200pf_obs_bind / b200pf_alert_bind)");
+    return 0;
+}
+
 static OppArgs env_opp(const b200pf_handle *h) {
     if (!h->opp_batch || h->opp_batch != h->env_batch) return OppArgs{};
     OppArgs o = h->opp;
@@ -1964,6 +1993,9 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
         return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
+    const AlertArgs al = env_alert(h);
+    int32_t *obs_rec; int obs_stride;
+    if (int rc0 = env_obs_record(h, al, &obs_rec, &obs_stride)) return rc0;
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2024,9 +2056,8 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     // 6. trips, isolated busbars, cooldowns, game over, the observe layer's input record
     a.status = h->x_status ? h->x_status : h->d_status;
     a.disc = h->prot ? h->d_disc : nullptr;
-    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
-    a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3; a.stamp = stamp;
-    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a);
+    a.obs_in = obs_rec; a.obs_stride = obs_stride; a.stamp = stamp;
+    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, al);
     CU(cudaGetLastError());
     h->env_steps++;
     return 0;
@@ -2039,15 +2070,17 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
         return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
         return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
+    const AlertArgs al = env_alert(h);
+    int32_t *obs_rec; int obs_stride;
+    if (int rc0 = env_obs_record(h, al, &obs_rec, &obs_stride)) return rc0;
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
     const size_t nt = (size_t)g.n_topo_in;
     EnvArgs a = h->env;
     a.reset_mask = d_mask; a.reset_rows = d_rows;
-    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
-    a.obs_in = obs ? h->d_obs_in : nullptr; a.obs_stride = g.n_line + g.n_sub + 3;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi);
+    a.obs_in = obs_rec; a.obs_stride = obs_stride;
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi, al);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2101,7 +2134,7 @@ extern "C" int b200pf_env_set_state(b200pf_handle *h, const int8_t *topo, const 
     if (cap_dirty) H2D(h->env.cap_dirty, cap_dirty, B);
     if (obs_reset) H2D(h->env.obs_reset, obs_reset, B);
     const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
-    const size_t rec = B * (size_t)(h->g.n_line + h->g.n_sub + 3) * 4;
+    const size_t rec = B * (size_t)(obs ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3) * 4;
     if (obs_in && obs) {
         if (h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));        // (b200pf_observe's copy into the same record has left)
         H2D(h->d_obs_in, obs_in, rec);
@@ -2386,6 +2419,105 @@ extern "C" int b200pf_opp_multi_set_state(b200pf_handle *h, const uint32_t *mt, 
     const void *src[6] = {mt, mt_pos, wait, dur, actr, fails};
     CU(cudaSetDevice(h->device));
     for (int k = 0; k < 6; ++k)
+        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
+    CU(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// the alert state buffers in the order of b200pf_alert_get_state / _set_state, and their bytes for a batch of B
+enum { ALERT_N_BUF = 12 };
+static void alert_buffers(const AlertArgs &al, void *p[ALERT_N_BUF]) {
+    void *q[ALERT_N_BUF] = {al.last_alert, al.already, al.tsl_alert, al.duration, al.tsl_attack, al.under_alert, al.was_used, al.total,
+                            al.ts_attack, al.launched, al.current, al.cur_id};
+    for (int k = 0; k < ALERT_N_BUF; ++k) p[k] = q[k];
+}
+static void alert_sizes(int n, int ring, size_t B, size_t out[ALERT_N_BUF]) {
+    const size_t bn = B * (size_t)n;
+    const size_t s[ALERT_N_BUF] = {bn, bn, bn * 4, bn * 4, bn * 4, bn * 4, bn * 4, B * 4, bn * ring, bn * ring, bn, B * 4};
+    for (int k = 0; k < ALERT_N_BUF; ++k) out[k] = s[k];
+}
+
+extern "C" int b200pf_alert_bind(b200pf_handle *h, const b200pf_alert_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    if (d->n_alert < 1 || d->n_alert > ALERT_MAX_LINES || !d->lines || d->window < 1 || !d->raise_alert || !d->reward_out)
+        return fail(B200PF_E_ARG, "bad alert description");
+    for (int k = 0; k < d->n_alert; ++k) {
+        if (d->lines[k] < 0 || d->lines[k] >= h->g.n_line) return fail(B200PF_E_ARG, "alertable line out of range");
+        for (int j = 0; j < k; ++j) if (d->lines[j] == d->lines[k]) return fail(B200PF_E_ARG, "alertable line listed twice");
+    }
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (void *p : h->alert_allocs) cudaFree(p);
+    h->alert_allocs.clear();
+    h->alert_batch = 0;
+    const size_t B = (size_t)h->env_batch;
+    AlertArgs al{};
+    al.n = d->n_alert; al.window = d->window; al.ring = d->window + 2; al.reward = d->reward ? 1 : 0;
+    al.min_blackout = (double)d->reward_min_blackout;
+    al.range_blackout = (double)(d->reward_max_blackout - d->reward_min_blackout);           // float32, as AlertReward
+    al.max_no_blackout = (double)d->reward_max_no_blackout;
+    al.diff_no_blackout = (double)(d->reward_min_no_blackout - d->reward_max_no_blackout);    // float32, as AlertReward
+    al.raise = d->raise_alert; al.reward_out = d->reward_out;
+    void *lines = nullptr;
+    CU(cudaMalloc(&lines, (size_t)al.n * 4));
+    h->alert_allocs.push_back(lines);
+    H2D(lines, d->lines, (size_t)al.n * 4);
+    al.lines = (const int32_t *)lines;
+    size_t sz[ALERT_N_BUF];
+    alert_sizes(al.n, al.ring, B, sz);
+    void *p[ALERT_N_BUF];
+    for (int k = 0; k < ALERT_N_BUF; ++k) {
+        CU(cudaMalloc(&p[k], sz[k]));
+        h->alert_allocs.push_back(p[k]);
+    }
+    al.last_alert = (uint8_t *)p[0]; al.already = (uint8_t *)p[1]; al.tsl_alert = (int32_t *)p[2]; al.duration = (int32_t *)p[3];
+    al.tsl_attack = (int32_t *)p[4]; al.under_alert = (int32_t *)p[5]; al.was_used = (int32_t *)p[6]; al.total = (int32_t *)p[7];
+    al.ts_attack = (uint8_t *)p[8]; al.launched = (uint8_t *)p[9]; al.current = (uint8_t *)p[10]; al.cur_id = (int32_t *)p[11];
+    // every instance starts from _reset_alert + AlertReward.reset: zeros, and -1 for the two "time since" counters
+    for (int k = 0; k < ALERT_N_BUF; ++k) CU(cudaMemsetAsync(p[k], (k == 2 || k == 4) ? 0xff : 0, sz[k], h->stream));
+    CU(cudaMemsetAsync(al.reward_out, 0, B * 8, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->alert = al; h->alert_batch = (int)B;
+    return 0;
+}
+
+static bool alert_bound(const b200pf_handle *h) { return env_bound(h) && h->alert_batch == h->env_batch; }
+
+extern "C" int b200pf_alert_get_state(b200pf_handle *h, uint8_t *last_alert, uint8_t *already, int32_t *tsl_alert, int32_t *duration,
+                                      int32_t *tsl_attack, int32_t *under_alert, int32_t *was_used, int32_t *total, uint8_t *ts_attack,
+                                      uint8_t *launched, uint8_t *current, int32_t *cur_id) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!alert_bound(h)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
+    CU(cudaSetDevice(h->device));
+    size_t sz[ALERT_N_BUF];
+    alert_sizes(h->alert.n, h->alert.ring, (size_t)h->alert_batch, sz);
+    void *src[ALERT_N_BUF];
+    alert_buffers(h->alert, src);
+    void *dst[ALERT_N_BUF] = {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack, launched,
+                              current, cur_id};
+    CU(cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < ALERT_N_BUF; ++k)
+        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
+    return 0;
+}
+
+extern "C" int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_alert, const uint8_t *already, const int32_t *tsl_alert,
+                                      const int32_t *duration, const int32_t *tsl_attack, const int32_t *under_alert, const int32_t *was_used,
+                                      const int32_t *total, const uint8_t *ts_attack, const uint8_t *launched, const uint8_t *current,
+                                      const int32_t *cur_id) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!alert_bound(h)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
+    const size_t B = (size_t)h->alert_batch;
+    if (cur_id) for (size_t i = 0; i < B; ++i) if (cur_id[i] < 0 || cur_id[i] >= h->alert.ring) return fail(B200PF_E_ARG, "ring index out of range");
+    CU(cudaSetDevice(h->device));
+    size_t sz[ALERT_N_BUF];
+    alert_sizes(h->alert.n, h->alert.ring, B, sz);
+    void *dst[ALERT_N_BUF];
+    alert_buffers(h->alert, dst);
+    const void *src[ALERT_N_BUF] = {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack, launched,
+                                    current, cur_id};
+    for (int k = 0; k < ALERT_N_BUF; ++k)
         if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
     CU(cudaStreamSynchronize(h->stream));
     return 0;

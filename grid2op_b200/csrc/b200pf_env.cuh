@@ -7,6 +7,8 @@
 //                        decision before the agent's action and its attack after the outages when one is bound (b200pf_opp.cuh);
 //   env_post_instance    the rest of BatchedEnv.step behind the solve;
 //   env_reset_instance   BatchedEnv.reset_instances (with the library's part, b200pf_series_reset_instances, and the opponent's).
+// With line alerts bound (b200pf_alert.cuh), the post body updates the alert state and the AlertReward after the step's attack,
+// and the reset body resets them.
 // The bodies are __host__ __device__: the CUDA launches run one thread per instance, a host build (tests/emu/env_emu.cpp,
 // tests/emu/opp_emu.cpp) runs the same source over the batch.  Integer arithmetic, and the opponent's fp64 operations explicitly
 // rounded: the two builds are bit-identical by construction.
@@ -15,6 +17,7 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "b200pf_alert.cuh"
 #include "b200pf_opp.cuh"
 
 #if defined(__CUDACC__)
@@ -260,8 +263,8 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     }
 }
 
-// the rest of BatchedEnv.step behind the solve, for instance i
-ENV_HD inline void env_post_instance(const EnvArgs &a, int i) {
+// the rest of BatchedEnv.step behind the solve, for instance i (al: NULL or the line alerts)
+ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *al = nullptr) {
     const int nl = a.n_line, ns = a.n_sub;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const bool live = a.done[i] == 0;
@@ -318,19 +321,29 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i) {
         a.is_illegal[i] = 0;
         if (live) { a.current_step[i] = 0; a.obs_reset[i] = 1; }
     } else if (live) a.current_step[i] += 1;
+    const bool alerts = al && al->n;
+    if (alerts) {                                             // an instance finished before the step keeps its alert state
+        if (live && !a.from_reset) {
+            alert_update_instance(*al, i);
+            if (al->reward) alert_reward_instance(*al, i, newly);
+            else al->reward_out[i] = 0.0;
+        } else al->reward_out[i] = 0.0;
+    }
     if (a.obs_in) {                                           // BatchedEnv.observe_inputs
         int32_t *h = a.obs_in + (size_t)i * a.obs_stride;
         for (int l = 0; l < nl; ++l) h[l] = lc[l];
         for (int s = 0; s < ns; ++s) h[nl + s] = sc[s];
         h[nl + ns] = a.current_step[i]; h[nl + ns + 1] = a.stamp;
         h[nl + ns + 2] = (a.is_illegal[i] ? 1 : 0) + (a.done[i] ? 2 : 0) + (a.obs_reset[i] ? 4 : 0);
+        if (alerts) alert_obs_record(*al, i, h + nl + ns + 3);
     }
 }
 
 // BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
 ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
-                                      const OppMultiArgs *m = nullptr) {
+                                      const OppMultiArgs *m = nullptr, const AlertArgs *al = nullptr) {
     if (!a.reset_mask[i]) return;
+    if (al && al->n) alert_reset_instance(*al, i);
     if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
     if (o && g && o->kind == OPP_GEOMETRIC) opp_geo_reset_instance(*o, *g, i);
     if (o && m && o->kind == OPP_GEOMETRIC_MULTI) opp_multi_reset_instance(*m, i);
@@ -360,6 +373,7 @@ ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o 
         int32_t *h = a.obs_in + (size_t)i * a.obs_stride;
         for (int j = 0; j < nl + a.n_sub + 1; ++j) h[j] = 0;
         h[nl + a.n_sub + 2] = 4;
+        if (al && al->n) alert_obs_record(*al, i, h + nl + a.n_sub + 3);
     }
 }
 
@@ -382,14 +396,15 @@ __global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o,
     env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a) {
+__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_post_instance(a, i);
+    if (i < a.batch) env_post_instance(a, i, al.n ? &al : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, AlertArgs al) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
+    if (i < a.batch)
+        env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr, al.n ? &al : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

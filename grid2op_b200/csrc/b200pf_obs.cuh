@@ -6,7 +6,7 @@
 //                        list of the environment's observation class (CompleteObservation.attr_list_vect, completeObservation.py:140-212,
 //                        or a subset); every attribute as float32, in the order given;
 //   reward               RedispReward (grid2op/Reward/redispReward.py:141-211) or L2RPNReward (l2RPNReward.py:52-77).
-// Without redispatching, curtailment, storage actions, alarms, alerts or detachment these attributes hold the values the
+// Without redispatching, curtailment, storage actions, alarms or detachment these attributes hold the values the
 // reference produces when the features are unused.  The overflow counters timestep_overflow / timestep_protection_engaged
 // (baseEnv.py:3361-3370, counted even under NO_OVERFLOW_DISCONNECTION) are kept here, per instance, because the series kernels
 // only count while their protections are on.
@@ -77,9 +77,10 @@ struct ObsArgs {
     int n_seg, n_obs;
     int reward_kind;
     double max_regret, reward_min, reward_illegal, dts_hours;
-    // per-instance host inputs: int32 [batch][host_stride] = cooldown_line[n_line] | cooldown_sub[n_sub] | current_step | stamp | flags
+    // per-instance host inputs: int32 [batch][host_stride] = cooldown_line[n_line] | cooldown_sub[n_sub] | current_step | stamp | flags,
+    // then with line alerts (n_alert > 0) the 6 n_alert + 1 alert values of alert_obs_record (b200pf_alert.cuh)
     const int32_t *host;
-    int host_stride;
+    int host_stride, n_alert;
     // device state of the observation layer
     int32_t *ts_over, *ts_prot;                         // [batch][n_line]
     int32_t *stamp;                                     // [batch]: host stamp of the step the counters were last advanced for
@@ -150,7 +151,16 @@ OBS_HD inline float obs_value(const ObsArgs &a, const ObsRec &R, int inst, int s
     }
     case OS_GEN_P_BEFORE_CURTAIL: return (go || !a.gen_renewable[j]) ? 0.f : rec[R.unit_p + a.n_hidden + j];   // renewables only
     case OS_CURTAILMENT_LIMIT: case OS_CURTAILMENT_LIMIT_EFFECTIVE: return 1.f;
-    case OS_TIME_SINCE_LAST_ALARM: case OS_TIME_SINCE_LAST_ATTACK: return -1.f;
+    case OS_TIME_SINCE_LAST_ALARM: return -1.f;
+    // line alerts (n_alert > 0): the game-over observation clears the alerts, their durations and the total, shows no attack,
+    // and keeps attack_under_alert / was_alert_used_after_attack (BaseObservation.set_game_over, then update_after_reward)
+    case OS_ACTIVE_ALERT: return go ? 0.f : (float)hin[a.n_line + a.n_sub + 3 + j];
+    case OS_ATTACK_UNDER_ALERT: return (float)hin[a.n_line + a.n_sub + 3 + a.n_alert + j];
+    case OS_TIME_SINCE_LAST_ALERT: return go ? 0.f : (float)hin[a.n_line + a.n_sub + 3 + 2 * a.n_alert + j];
+    case OS_ALERT_DURATION: return go ? 0.f : (float)hin[a.n_line + a.n_sub + 3 + 3 * a.n_alert + j];
+    case OS_TOTAL_NUMBER_OF_ALERT: return go ? 0.f : (float)hin[a.n_line + a.n_sub + 3 + 4 * a.n_alert];
+    case OS_TIME_SINCE_LAST_ATTACK: return go ? -1.f : (float)hin[a.n_line + a.n_sub + 4 + 4 * a.n_alert + j];
+    case OS_WAS_ALERT_USED_AFTER_ATTACK: return (float)hin[a.n_line + a.n_sub + 4 + 5 * a.n_alert + j];
     case OS_SHUNT_P: return go ? 0.f : rec[R.sh_p + j];
     case OS_SHUNT_Q: return go ? 0.f : rec[R.sh_q + j];
     case OS_SHUNT_V: return go ? 0.f : rec[R.sh_v + j];
@@ -168,7 +178,7 @@ OBS_HD inline float obs_value(const ObsArgs &a, const ObsRec &R, int inst, int s
     }
     case OS_GEN_P_DELTA: return go ? 0.f : rec[R.unit_p + a.n_hidden + j] - crow[2 * a.n_load + j];
     case OS_TS_PROTECTION_ENGAGED: return go ? 0.f : (float)tspr[j];
-    default: return 0.f;          // dispatch, storage power, curtailment, alarms, alerts, detachment: features unused
+    default: return 0.f;          // dispatch, storage power, curtailment, alarms, detachment: features unused
     }
 }
 

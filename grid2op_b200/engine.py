@@ -42,6 +42,7 @@ ABI_SYMBOLS = (
     "b200pf_opp_bind", "b200pf_opp_get_state", "b200pf_opp_set_state",
     "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
     "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state",
+    "b200pf_alert_bind", "b200pf_alert_get_state", "b200pf_alert_set_state",
 )
 
 
@@ -76,7 +77,7 @@ class ObsDesc(C.Structure):
         ("gen_cost", C.c_void_p), ("gen_renewable", C.c_void_p), ("redisp_available", C.c_int32),
         ("sto_charge0", C.c_void_p), ("sto_loss_step", C.c_void_p), ("reward_kind", C.c_int32),
         ("max_regret", C.c_double), ("reward_min", C.c_double), ("reward_illegal", C.c_double), ("dts_hours", C.c_double),
-        ("soft_thr", C.c_float),
+        ("soft_thr", C.c_float), ("n_alert", C.c_int32),
     ]
 
 
@@ -118,6 +119,15 @@ class OppMultiDesc(C.Structure):
         ("logq_hazard", C.c_double), ("logq_recovery", C.c_double), ("recovery_min", C.c_int32), ("cap", C.c_int32),
         ("episode_max_time", C.c_void_p), ("mt", C.c_void_p), ("mt_pos", C.c_void_p), ("wait", C.c_void_p), ("dur", C.c_void_p),
         ("actr", C.c_void_p), ("fails", C.c_void_p), ("attack_lines", C.c_void_p),
+    ]
+
+
+class AlertDesc(C.Structure):
+    """``b200pf_alert_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("n_alert", C.c_int32), ("lines", C.c_void_p), ("window", C.c_int32), ("reward", C.c_int32),
+        ("reward_min_no_blackout", C.c_float), ("reward_min_blackout", C.c_float), ("reward_max_no_blackout", C.c_float),
+        ("reward_max_blackout", C.c_float), ("raise_alert", C.c_void_p), ("reward_out", C.c_void_p),
     ]
 
 
@@ -184,6 +194,7 @@ def make_obs_desc(t: dict):
     r = t["reward"]
     d.max_regret, d.reward_min, d.reward_illegal, d.dts_hours = r["max_regret"], r["reward_min"], r["reward_illegal"], r["dts_hours"]
     d.soft_thr = float(t["soft_thr"])
+    d.n_alert = int(t.get("n_alert", 0))
     return d, keep
 
 
@@ -292,10 +303,14 @@ def load_library():
     lib.b200pf_opp_multi_bind.argtypes = [vp, C.POINTER(OppMultiDesc)]
     lib.b200pf_opp_multi_get_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.b200pf_opp_multi_set_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.b200pf_alert_bind.argtypes = [vp, C.POINTER(AlertDesc)]
+    lib.b200pf_alert_get_state.argtypes = [vp] + [vp] * 12
+    lib.b200pf_alert_set_state.argtypes = [vp] + [vp] * 12
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
                "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
-               "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state"):
+               "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state", "b200pf_alert_bind",
+               "b200pf_alert_get_state", "b200pf_alert_set_state"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -747,7 +762,7 @@ class PowerFlowEngine:
         b = None if nb_inst is None else np.ascontiguousarray(nb_inst, np.int32)
         c = None if cap_dirty is None else np.ascontiguousarray(cap_dirty, np.uint8)
         r = None if obs_reset is None else np.ascontiguousarray(obs_reset, np.uint8)
-        o = None if obs_in is None else np.ascontiguousarray(obs_in, np.int32).reshape(B, gm.n_line + gm.n_sub + 3)
+        o = None if obs_in is None else np.ascontiguousarray(obs_in, np.int32).reshape(B, -1)
         self._check(self.lib.b200pf_env_set_state(self.h, _ptr(a), _ptr(b), _ptr(c), _ptr(r), _ptr(o)), "b200pf_env_set_state")
 
     def env_pointers(self):
@@ -840,6 +855,33 @@ class PowerFlowEngine:
     def opp_multi_set_state(self, s: dict):
         a = [np.ascontiguousarray(s[k], dt) for k, dt in _MULTI_STATE]
         self._check(self.lib.b200pf_opp_multi_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_multi_set_state")
+
+    def alert_bind(self, a, d_raise: int, d_reward: int):
+        """line alerts of the device environment (``b200pf_alert_bind``): ``a`` a :class:`grid2op_b200.alert.BatchedAlerts` (lines,
+        window, constants), caller-owned device buffers uint8 [B, n] (the step's raise_alert) and float64 [B] (AlertReward)"""
+        lines = np.ascontiguousarray(a.lines, np.int32)
+        c = a.constants
+        d = AlertDesc(n_alert=len(lines), lines=lines.ctypes.data, window=int(a.window), reward=int(a.reward),
+                      reward_min_no_blackout=float(c["reward_min_no_blackout"]), reward_min_blackout=float(c["reward_min_blackout"]),
+                      reward_max_no_blackout=float(c["reward_max_no_blackout"]), reward_max_blackout=float(c["reward_max_blackout"]),
+                      raise_alert=int(d_raise), reward_out=int(d_reward))
+        self._check(self.lib.b200pf_alert_bind(self.h, C.byref(d)), "b200pf_alert_bind")
+        self._alert_shape = (len(lines), int(a.ring))
+
+    def alert_get_state(self):
+        """-> the alert state of every instance, the arrays of :data:`grid2op_b200.alert.ALERT_STATE`"""
+        from .alert import ALERT_STATE
+        B = self._series_batch
+        n, R = getattr(self, "_alert_shape", (0, 0))                        # (unbound: the library refuses the call)
+        s = {k: np.empty((B,) if k in ("total", "cur_id") else (B, R, n) if k in ("ts_attack", "launched") else (B, n), dt)
+             for k, dt in ALERT_STATE}
+        self._check(self.lib.b200pf_alert_get_state(self.h, *[_ptr(s[k]) for k, _ in ALERT_STATE]), "b200pf_alert_get_state")
+        return s
+
+    def alert_set_state(self, s: dict):
+        from .alert import ALERT_STATE
+        a = [np.ascontiguousarray(s[k], dt) for k, dt in ALERT_STATE]
+        self._check(self.lib.b200pf_alert_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_alert_set_state")
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")

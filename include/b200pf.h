@@ -306,7 +306,9 @@ int64_t b200pf_redo_launch_count(const b200pf_handle *h);
  * n_sub + 3) bytes per instance.  The counters advance once per distinct stamp (the caller's step number): observe after every
  * step.  flags: B200PF_OBS_ILLEGAL (the step's action was replaced by "do nothing"), B200PF_OBS_DONE (the instance is game over:
  * the game-over observation of BaseObservation.set_game_over, baseObservation.py:1551, and reward_min), B200PF_OBS_RESET (the
- * instance was reset: its counters restart from 0). */
+ * instance was reset: its counters restart from 0).  With line alerts (n_alert > 0, b200pf_alert_bind) the record of an instance
+ * continues with 6 n_alert + 1 int32: active_alert | attack_under_alert | time_since_last_alert | alert_duration |
+ * total_number_of_alert | time_since_last_attack | was_alert_used_after_attack, and the alert attributes of `seg` read them. */
 enum { B200PF_REWARD_NONE = 0, B200PF_REWARD_REDISP = 1, B200PF_REWARD_L2RPN = 2 };
 enum { B200PF_OBS_ILLEGAL = 1, B200PF_OBS_DONE = 2, B200PF_OBS_RESET = 4 };
 typedef struct b200pf_obs_desc {
@@ -323,6 +325,7 @@ typedef struct b200pf_obs_desc {
     int32_t reward_kind;                /* B200PF_REWARD_* */
     double max_regret, reward_min, reward_illegal, dts_hours;   /* RedispReward constants; step length in hours */
     float soft_thr;                     /* SOFT_OVERFLOW_THRESHOLD (timestep_protection_engaged) */
+    int32_t n_alert;                    /* dim_alerts: alert values in the host record (0: none, the record as without alerts) */
 } b200pf_obs_desc;
 int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *desc);
 int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float *d_reward);
@@ -474,6 +477,36 @@ int b200pf_opp_multi_bind(b200pf_handle *h, const b200pf_opp_multi_desc *desc);
 int b200pf_opp_multi_get_state(b200pf_handle *h, uint32_t *mt, int32_t *mt_pos, int32_t *wait, int32_t *dur, int32_t *actr, int32_t *fails);
 int b200pf_opp_multi_set_state(b200pf_handle *h, const uint32_t *mt, const int32_t *mt_pos, const int32_t *wait, const int32_t *dur,
                                const int32_t *actr, const int32_t *fails);
+
+/* Line alerts of the device environment (grid2op's alerts of l2rpn_idf_2023, csrc/b200pf_alert.cuh), after b200pf_env_bind.
+ * b200pf_alert_bind copies the alertable lines (host, n_alert <= 64, in grid2op's order) and the constants, allocates the
+ * per-instance state in the library and sets every instance to BaseEnv._reset_alert + AlertReward.reset.  From then on the post
+ * launch of b200pf_env_step updates, for every instance live before the step and not on a reset step, the environment's alert
+ * state (BaseEnv._update_alert_properties, with the attacked lines of the opponent bound by b200pf_opp_bind / _multi_bind, none
+ * without an opponent) and, when `reward`, the AlertReward into reward_out (float64 [batch], caller-owned device buffer; 0 for
+ * the other instances).  raise_alert: caller-owned DEVICE uint8 [batch][n_alert] the caller fills before each step (0 / 1).
+ * b200pf_env_reset resets the alert state of the reset instances.  With the observation layer bound with the same n_alert, the
+ * post and reset launches write the alert values into the observe input record.  get_state / set_state copy the whole state
+ * between the device and host arrays (any pointer may be NULL): last_alert / already uint8 [batch][n], tsl_alert / duration /
+ * tsl_attack / under_alert / was_used int32 [batch][n], total / cur_id int32 [batch], ts_attack / launched uint8
+ * [batch][window + 2][n], current uint8 [batch][n] (AlertReward._ts_attack, _alert_launched, _lines_currently_attacked). */
+typedef struct b200pf_alert_desc {
+    int32_t n_alert;                    /* dim_alerts, 1..64 */
+    const int32_t *lines;               /* [n_alert] alertable line ids */
+    int32_t window;                     /* ALERT_TIME_WINDOW, >= 1 */
+    int32_t reward;                     /* compute AlertReward (and was_alert_used_after_attack) */
+    float reward_min_no_blackout, reward_min_blackout, reward_max_no_blackout, reward_max_blackout;
+    const uint8_t *raise_alert;         /* device [batch][n_alert] step input */
+    double *reward_out;                 /* device [batch] per-step output */
+} b200pf_alert_desc;
+int b200pf_alert_bind(b200pf_handle *h, const b200pf_alert_desc *desc);
+int b200pf_alert_get_state(b200pf_handle *h, uint8_t *last_alert, uint8_t *already, int32_t *tsl_alert, int32_t *duration,
+                           int32_t *tsl_attack, int32_t *under_alert, int32_t *was_used, int32_t *total, uint8_t *ts_attack,
+                           uint8_t *launched, uint8_t *current, int32_t *cur_id);
+int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_alert, const uint8_t *already, const int32_t *tsl_alert,
+                           const int32_t *duration, const int32_t *tsl_attack, const int32_t *under_alert, const int32_t *was_used,
+                           const int32_t *total, const uint8_t *ts_attack, const uint8_t *launched, const uint8_t *current,
+                           const int32_t *cur_id);
 
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */

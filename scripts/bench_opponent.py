@@ -8,7 +8,10 @@ environments' constants with a small initial budget, so that attacks run from th
 synchronise, after warm-up.  Prints env.step/s (min / median / max over the repeats), the extra bytes per step the opponent moves, and
 the card and its power limit read in the same run.
 
-    python scripts/bench_opponent.py [--steps 50] [--warmup 5] [--repeats 5]
+With ``--alerts``: l2rpn_idf_2023 at batch 1024 with its multi-area opponent in both runs, protections off, line alerts off and
+on (``enable_alerts`` on the opponent's 22 lines, a random alert tensor drawn on the GPU every step), alternating in one process.
+
+    python scripts/bench_opponent.py [--steps 50] [--warmup 5] [--repeats 5] [--alerts]
 """
 import argparse
 import os
@@ -49,7 +52,8 @@ OPPONENTS = {
 }
 
 
-def run(name, B, protections, steps, warmup, repeats):
+def run(name, B, protections, steps, warmup, repeats, alerts=False):
+    """``alerts``: both environments run the opponent, the second one also the line alerts (the comparison is alerts off / on)"""
     import torch
     from bench_env_tensor import draw
     from conftest import env_grid
@@ -66,11 +70,13 @@ def run(name, B, protections, steps, warmup, repeats):
     envs = {}
     for mode in ("off", "on"):
         e = BatchedEnv(gm, chron, B, nb_timestep_cooldown_line=2, nb_timestep_cooldown_sub=2, protections=protections)
+        if alerts and mode == "on":
+            e.enable_alerts(OPPONENTS[name]["lines"])
         e.enable_observation(env_dir, scenarios=folders)
         if protections:
             e.engine.set_kernel_policy(e.engine.KERNEL_PLANNED)
         e.step_tensors(from_reset=True)
-        if mode == "on":
+        if mode == "on" or alerts:
             o = dict(OPPONENTS[name])
             e.enable_opponent(o.pop("kind"), o.pop("lines"), seeds=[opponent_seed(s) for s in range(B)], **o)
         envs[mode] = e
@@ -79,9 +85,18 @@ def run(name, B, protections, steps, warmup, repeats):
         g.manual_seed(0)
     attacks = {m: 0 for m in envs}
 
+    n_alert = envs["on"]._alerts.n if alerts else 0
+
     def one(mode, count=False):
         e = envs[mode]
-        _, done, info = e.step_tensors(*draw(e, gens[mode], dev))
+        act = draw(e, gens[mode], dev)
+        if mode == "on" and alerts:              # (drawn in both modes, so that both streams draw the same actions)
+            up = torch.rand((B, n_alert), device=dev, generator=gens[mode]) < 0.3
+            _, done, info = e.step_tensors(*act, raise_alert=up)
+        else:
+            if alerts:
+                torch.rand((B, n_alert), device=dev, generator=gens[mode])
+            _, done, info = e.step_tensors(*act)
         e.observe()
         e.reset_instances(done.clone())
         if count and "opponent_attack_line" in info:
@@ -108,7 +123,7 @@ def run(name, B, protections, steps, warmup, repeats):
     one("on", count=True)
     for m in ("off", "on"):
         r = np.array([x[0] for x in res[m]])
-        print(f"{name:28s} B={B:5d} prot={int(protections)} opponent {m:3s}: env.step/s min {r.min():.3e} median {np.median(r):.3e} "
+        print(f"{name:28s} B={B:5d} prot={int(protections)} {'alerts' if alerts else 'opponent'} {m:3s}: env.step/s min {r.min():.3e} median {np.median(r):.3e} "
               f"max {r.max():.3e}; bytes moved per step {np.median([x[1] for x in res[m]]) / 1e3:.1f} kB")
     print(f"{'':28s} attacks running in the last step: {attacks['on']} of {B}")
     for e in envs.values():
@@ -122,8 +137,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--only", default=None, help="one workload (environment name)")
+    ap.add_argument("--alerts", action="store_true", help="l2rpn_idf_2023 with its opponent, line alerts off / on")
     args = ap.parse_args()
     print("card, power limit:", card())
+    if args.alerts:
+        run("l2rpn_idf_2023", 1024, False, args.steps, args.warmup, args.repeats, alerts=True)
+        return
     for name, B in (("l2rpn_case14_sandbox", 4096), ("l2rpn_neurips_2020_track1", 1024), ("l2rpn_wcci_2022_dev", 1024),
                     ("l2rpn_idf_2023", 1024)):
         if args.only and name != args.only:
