@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -31,6 +32,9 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
             return fail(B200PF_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e__));     \
     } while (0)
 
+// kernel family of a launch, as b200pf_plan_stats reports it
+enum LaunchKind { KERN_NONE = 0, KERN_WARP_PIVOTING = 1, KERN_CTA_PIVOTING = 2, KERN_PLANNED_SPARSE = 3, KERN_PLANNED_BLOCK = 4 };
+
 struct b200pf_handle {
     int device = 0;
     int max_batch = 0;
@@ -43,7 +47,6 @@ struct b200pf_handle {
     bool group_pending[B200PF_MAX_GROUPS] = {};
     int small_occ[2][33] = {};
     int group_flags = 0;                                    // bit 0: kernels store results straight into pinned host memory
-    int env_flags = -1;                                     // bit 0: B200PF_JACOBIAN_FP64, bit 1: B200PF_NO_SMALL_KERNEL
     float *x_out = nullptr; int *x_status = nullptr; int *x_iters = nullptr; float *x_rho = nullptr;
     DevGrid g{};
     std::vector<void *> dev_allocs;
@@ -81,15 +84,15 @@ struct b200pf_handle {
     int plan_policy = 0;                                    // 0 auto, 1 never, 2 whenever a host copy of the topology exists
     int plan_max_smem = 0, plan_max_nb = 0, plan_max_nblkA = 0;
     int series_lay_nb = 0, series_lay_nblkA = 0;
-    int sparse_occ_smem = -1, sparse_occ = 0, sparse_occ_variant = 0;
+    const void *sparse_occ_kern = nullptr; int sparse_occ_smem = -1, sparse_occ = 0;   // planned kernels: last occupancy query
     int sparse_cta_cap = 0;                                 // > 0: resident CTAs per SM of the planned kernel are capped (rest of the SM's memory = L1); < 0: never
     int sparse_minb = 32;                                   // tuning: one-warp CTAs per SM the small-workspace variant is compiled for (32 or 28)
     int plan_T = 32;                                        // threads per instance of the planned kernel (32, 64, 128)
     int blk = 1;                                            // 1: BLOCK plans + pf_kernel_block (default), 0: scalar plans + pf_kernel_sparse
     int blk_T = 4, blk_U = 2;                               // lanes per instance / operations per lane and row of the block kernel
-    int blk_wpc = 4, blk_stage = 1, blk_minb = 16, blk_uni = 1, blk_wpc_pinned = 0, blk_spec = 1;
-    unsigned char *d_stat = nullptr; PlanArgs::StatOff stat_off{}; bool stat_dirty = true;   // packed static arrays for staged launches                         // experiment knobs: warps per CTA, TMA staging of a shared plan
-    int last_kernel = 0;                                    // 1 small, 2 generic, 3 sparse
+    int blk_wpc = 4, blk_stage = 1, blk_uni = 1, blk_wpc_pinned = 0, blk_spec = 1;   // experiment knobs: warps per CTA, TMA staging of a shared plan
+    unsigned char *d_stat = nullptr; PlanArgs::StatOff stat_off{}; bool stat_dirty = true;   // packed static arrays for staged launches
+    int last_kernel = KERN_NONE;                            // LaunchKind of the last launch (b200pf_plan_stats)
     int64_t plans_built = 0, plan_cache_resets = 0, plan_lookups = 0, plan_hits = 0;
     bool series_dev_topo_ahead = false;                     // the warp kernel tripped lines in d_series_topo on the device: the host mirror / plans lag
     bool series_plans_stale = false;                        // the cache was reset under the series' plan ids: re-resolve before the next step
@@ -394,41 +397,69 @@ extern "C" int b200pf_grid_max_active_buses(const b200pf_grid_desc *gd, int n, c
 // ------------------------------------------------------------------------------------------------
 // launch configuration
 // ------------------------------------------------------------------------------------------------
-// template parameters of the launch just issued, in the order of b200pf_last_launch_config (missing ones: -1)
-static void set_last_cfg(b200pf_handle *h, std::initializer_list<int> cfg) {
+// Raises a kernel's dynamic shared-memory limit to at least `bytes`.  The attribute belongs to the function, not to a handle
+// (launches from the device and every other handle see it too), so it is only ever raised: a larger limit never hurts, and
+// lowering it would break another handle's launch of a larger workspace.  The record of what was set is per device and
+// kernel and shared by all handles: setting the attribute on every launch kept the GPU waiting for the host between steps.
+static int raise_smem_limit(const b200pf_handle *h, const void *kern, int bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void *>, int> done;   // (device, kernel) -> largest limit set
+    std::lock_guard<std::mutex> lock(mu);
+    int &cur = done[{h->device, kern}];
+    if (bytes > cur) {
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        cur = bytes;
+    }
+    return 0;
+}
+
+// Grid of a persistent launch over `work` items (instances, or CTAs' worth of them) with `resident` CTAs on the device at
+// once, sized so that every CTA gets the same number of items (no ragged last wave): rounds = ceil(work / resident),
+// grid = ceil(work / rounds)
+static int balanced_grid(int work, int resident) {
+    const int rounds = (work + resident - 1) / resident;
+    const int grid = rounds > 0 ? (work + rounds - 1) / rounds : 1;
+    return grid < 1 ? 1 : grid;
+}
+
+// Bookkeeping of the launch just issued (b200pf_launch_count, b200pf_plan_stats, b200pf_last_launch_info), with its
+// template parameters in the order of b200pf_last_launch_config (missing ones: -1).  Returns the launch error, if any.
+static int launched(b200pf_handle *h, LaunchKind kind, int smem, int T, int grid, int block, std::initializer_list<int> cfg = {}) {
+    CU(cudaGetLastError());
+    h->launches++;
+    h->last_kernel = kind; h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = block;
     int k = 0;
     for (int v : cfg) h->last_cfg[k++] = v;
     for (; k < 8; ++k) h->last_cfg[k] = -1;
+    return 0;
 }
 
-template <int T, typename JT>
+// threads per instance of the pivoting kernels for a Newton system of dimension d: the big systems are latency bound -> many
+// warps per instance
+static int pivot_threads(size_t d) { return d <= 64 ? 32 : (d <= 128 ? 128 : (d <= 256 ? 256 : 512)); }
+
+// The warp-per-instance kernel (b200pf_small.cuh) takes a launch when every element class fits one warp and at most `cap`
+// <= 17 buses are active (a Newton system of <= 32 unknowns)
+static bool warp_kernel_fits(const DevGrid &g, int cap) {
+    return g.n_slot <= 32 && g.n_line <= 32 && g.n_unit <= 32 && g.n_load <= 32 && g.n_sto <= 32 && g.n_shunt <= 32 && cap <= 17;
+}
+
+template <int T>
 static int launch_t(b200pf_handle *h, const RunArgs &a) {
     const DevGrid &g = h->g;
-    constexpr int BLOCK = T;
-    constexpr int GPB = 1;
     WsLayout L = ws_layout(a.nb_cap, g.n_slot, g.n_line, g.n_inj, (size_t)a.mat_bytes);
-    const int ws_bytes = (int)L.total;
-    const size_t smem = (size_t)ws_bytes * GPB;
-    if (smem > (size_t)h->max_smem_optin)
+    const int smem = (int)L.total;
+    if (L.total > (size_t)h->max_smem_optin)
         return fail(B200PF_E_CAPACITY, "workspace does not fit in shared memory");
-    auto kern = pf_kernel<T, JT>;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    auto kern = pf_kernel<T, float>;
+    int rc = raise_smem_limit(h, (const void *)kern, smem);
+    if (rc) return rc;
     int occ = 1;
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, BLOCK, smem));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, T, (size_t)smem));
     if (occ < 1) occ = 1;
-    // persistent groups; size the grid so that every group gets the same number of instances (no
-    // ragged last wave): rounds = ceil(batch / resident groups), grid = ceil(batch / rounds)
-    int need = (a.batch + GPB - 1) / GPB;
-    int resident = h->sm_count * occ;
-    int rounds = (need + resident - 1) / resident;
-    int grid = (need + rounds - 1) / rounds;
-    if (grid < 1) grid = 1;
-    kern<<<grid, BLOCK, smem, h->stream>>>(g, a, ws_bytes);
-    CU(cudaGetLastError());
-    h->launches++;
-    h->last_smem = (int)smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 2;
-    set_last_cfg(h, {});
-    return 0;
+    const int grid = balanced_grid(a.batch, h->sm_count * occ);
+    kern<<<grid, T, (size_t)smem, h->stream>>>(g, a, smem);
+    return launched(h, KERN_CTA_PIVOTING, smem, T, grid, T);
 }
 
 // Sizing policy.  nb_cap (bus arrays) = the caller's bound or every slot.  The matrix region gets
@@ -436,28 +467,20 @@ static int launch_t(b200pf_handle *h, const RunArgs &a) {
 // ACTUAL system size of each instance against it (B200PF_ST_TOO_LARGE), so e.g. the 118-substation
 // grid (236 slots) runs as long as its Newton system (191 unknowns + splits) fits.
 static int launch_small(b200pf_handle *h, RunArgs a, int cap) {
-    const DevGrid &g = h->g;
     a.nb_cap = cap;
     SmallLayout L = small_layout(cap);
     a.mat_bytes = L.total - L.off_mat;
     auto kern = a.prot ? pf_kernel_small<true> : pf_kernel_small<false>;
     int &occ = h->small_occ[a.prot ? 1 : 0][cap];          // launch configuration cached per (variant, capacity)
     if (occ == 0) {
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+        int rc = raise_smem_limit(h, (const void *)kern, L.total);
+        if (rc) return rc;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32, (size_t)L.total));
         if (occ < 1) occ = 1;
     }
-    const int resident = h->sm_count * occ;
-    const int rounds = (a.batch + resident - 1) / resident;
-    int grid = (a.batch + rounds - 1) / rounds;
-    if (grid < 1) grid = 1;
-    kern<<<grid, 32, L.total, h->stream>>>(g, a, L);
-    CU(cudaGetLastError());
-    h->launches++;
-    h->last_smem = L.total; h->last_T = 32; h->last_grid = grid; h->last_block = 32; h->last_kernel = 1;
-    set_last_cfg(h, {});
-    (void)g;
-    return 0;
+    const int grid = balanced_grid(a.batch, h->sm_count * occ);
+    kern<<<grid, 32, L.total, h->stream>>>(h->g, a, L);
+    return launched(h, KERN_WARP_PIVOTING, L.total, 32, grid, 32);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -590,9 +613,7 @@ static int plan_cache_clear(b200pf_handle *h) {
 // Plans of the instances [0, n_src) whose topology rows are at host_topo (times n1_lines outages each in contingency
 // mode); ids go to h_inst_plan[first ...] and, unless all are equal, to d_inst_plan[first ...] on stream st.
 // Returns 1 = use the sparse kernel with *sel, 0 = fall back to the pivoting kernels, < 0 error.
-static int plan_select(b200pf_handle *h, const int8_t *host_topo, int n_src, int n1_lines, int first, cudaStream_t st, PlanSel *sel,
-                       int nb_cap) {
-    (void)nb_cap;
+static int plan_select(b200pf_handle *h, const int8_t *host_topo, int n_src, int n1_lines, int first, cudaStream_t st, PlanSel *sel) {
     if (h->plan_policy == 1 || !host_topo) return 0;
     const DevGrid &g = h->g;
     const size_t nt = (size_t)g.n_topo_in;
@@ -704,43 +725,45 @@ static int plan_select(b200pf_handle *h, const int8_t *host_topo, int n_src, int
     return 1;
 }
 
+// Resident CTAs per SM of a planned kernel (scalar or block) with `smem` bytes of dynamic shared memory per CTA, in
+// h->sparse_occ.  One entry per handle, re-queried when the kernel or the workspace changes: the carveout set here changes
+// what the next query returns.  `smem_limit` is the kernel's dynamic shared-memory limit; auto_cap lets a large workspace cap
+// the resident CTAs by itself.
+static int planned_occupancy(b200pf_handle *h, const void *kern, int block, int smem, int smem_limit, bool auto_cap) {
+    if (h->sparse_occ_kern == kern && h->sparse_occ_smem == smem) return 0;
+    int rc = raise_smem_limit(h, kern, smem_limit);
+    if (rc) return rc;
+    int occ = 1;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, block, (size_t)smem));
+    if (occ < 1) occ = 1;
+    int cap = h->sparse_cta_cap;
+    if (cap == 0 && auto_cap && smem >= 16 * 1024) cap = (164 * 1024) / (smem + 1024);   // large workspaces (118 substations): leave ~90 KB of L1 (measured +10%)
+    if (cap > 0 && occ > cap) {
+        // fewer resident instances, more L1: the plan arrays (operation stream, positions, line data) are re-read by
+        // every instance and every Newton iteration; what shared memory does not take is L1 for them
+        occ = cap;
+        int pct = (int)(((size_t)occ * (size_t)(smem + 1024) * 100 + (size_t)h->max_smem_optin - 1) / (size_t)h->max_smem_optin);
+        if (pct > 100) pct = 100;
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    }
+    h->sparse_occ = occ; h->sparse_occ_kern = kern; h->sparse_occ_smem = smem;
+    return 0;
+}
+
 template <int T, int MINB, bool PROT = false>
-static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd, int variant) {
-    const DevGrid &g = h->g;
+static int launch_sparse_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd) {
     auto kern = pf_kernel_sparse<T, MINB, PROT>;
     const int smem = sel.smem;
-    if (h->sparse_occ_smem != smem || h->sparse_occ_variant != variant) {
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->max_smem_optin));
-        int occ = 1;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, T, (size_t)smem));
-        if (occ < 1) occ = 1;
-        int cap = h->sparse_cta_cap;
-        if (cap == 0 && smem >= 16 * 1024) cap = (164 * 1024) / (smem + 1024);   // large workspaces (118 substations): leave ~90 KB of L1 (measured +10%)
-        if (cap > 0 && occ > cap) {
-            // fewer resident instances, more L1: the plan arrays (operation stream, positions, line data) are re-read by
-            // every instance and every Newton iteration; what shared memory does not take is L1 for them
-            occ = cap;
-            int pct = (int)(((size_t)occ * (size_t)(smem + 1024) * 100 + (size_t)h->max_smem_optin - 1) / (size_t)h->max_smem_optin);
-            if (pct > 100) pct = 100;
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
-        }
-        h->sparse_occ = occ; h->sparse_occ_smem = smem; h->sparse_occ_variant = variant;
-    }
+    int rc = planned_occupancy(h, (const void *)kern, T, smem, h->max_smem_optin, true);
+    if (rc) return rc;
     PlanArgs pa{};
     pa.blobs = h->d_plan_blobs;
     pa.plan_off = h->d_plan_off + (sel.d_inst_plan ? 0 : sel.single);
     pa.inst_plan = sel.d_inst_plan;
     pa.lay_nb = 0; pa.lay_nblkA = 0;
-    const int resident = h->sm_count * h->sparse_occ;
-    const int rounds = (a.batch + resident - 1) / resident;
-    int grid = (a.batch + rounds - 1) / rounds;
-    if (grid < 1) grid = 1;
-    kern<<<grid, T, (size_t)smem, h->stream>>>(g, a, pa, rd);
-    CU(cudaGetLastError());
-    h->launches++;
-    h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = T; h->last_kernel = 3;
-    set_last_cfg(h, {T, -1, MINB, PROT ? 1 : 0});
-    return 0;
+    const int grid = balanced_grid(a.batch, h->sm_count * h->sparse_occ);
+    kern<<<grid, T, (size_t)smem, h->stream>>>(h->g, a, pa, rd);
+    return launched(h, KERN_PLANNED_SPARSE, smem, T, grid, T, {T, -1, MINB, PROT ? 1 : 0});
 }
 
 // Threads per instance (fixed per handle: the plans' operation streams are laid out for it) and register budget of the
@@ -752,17 +775,17 @@ static int launch_sparse(b200pf_handle *h, const RunArgs &a, const PlanSel &sel,
     if (h->blk) return launch_block(h, a, sel, rd);
     const int per_sm = h->max_smem_optin / (sel.smem + 1024);
     if (a.prot) {     // protections: one launch per cascade round, see series_step_planned_prot
-        if (h->plan_T == 128) return launch_sparse_t<128, 4, true>(h, a, sel, rd, 14);
-        if (h->plan_T == 64) return launch_sparse_t<64, 10, true>(h, a, sel, rd, 15);
-        return launch_sparse_t<32, 16, true>(h, a, sel, rd, 13);
+        if (h->plan_T == 128) return launch_sparse_t<128, 4, true>(h, a, sel, rd);
+        if (h->plan_T == 64) return launch_sparse_t<64, 10, true>(h, a, sel, rd);
+        return launch_sparse_t<32, 16, true>(h, a, sel, rd);
     }
-    if (h->plan_T == 128) return launch_sparse_t<128, 4>(h, a, sel, rd, 4);
-    if (h->plan_T == 64) return launch_sparse_t<64, 10>(h, a, sel, rd, 5);
-    if (per_sm >= 32 && h->sparse_minb == 28) return launch_sparse_t<32, 28>(h, a, sel, rd, 7);   // 73 registers, 4144 resident warps
-    if (per_sm >= 32) return launch_sparse_t<32, 32>(h, a, sel, rd, 1);
-    if (per_sm >= 24) return launch_sparse_t<32, 24>(h, a, sel, rd, 2);
-    if (per_sm >= 16) return launch_sparse_t<32, 16>(h, a, sel, rd, 3);
-    return launch_sparse_t<32, 8>(h, a, sel, rd, 6);
+    if (h->plan_T == 128) return launch_sparse_t<128, 4>(h, a, sel, rd);
+    if (h->plan_T == 64) return launch_sparse_t<64, 10>(h, a, sel, rd);
+    if (per_sm >= 32 && h->sparse_minb == 28) return launch_sparse_t<32, 28>(h, a, sel, rd);   // 73 registers, 4144 resident warps
+    if (per_sm >= 32) return launch_sparse_t<32, 32>(h, a, sel, rd);
+    if (per_sm >= 24) return launch_sparse_t<32, 24>(h, a, sel, rd);
+    if (per_sm >= 16) return launch_sparse_t<32, 16>(h, a, sel, rd);
+    return launch_sparse_t<32, 8>(h, a, sel, rd);
 }
 
 // Sizing of the generic pivoting kernel for nb_cap active buses: threads per instance, matrix bytes (see the policy above
@@ -771,14 +794,9 @@ static int generic_config(b200pf_handle *h, int cap, int jt, int *T_out, size_t 
     const DevGrid &g = h->g;
     const size_t fixed = ws_fixed_bytes(cap, g.n_slot, g.n_line, g.n_inj);
     size_t want = ws_mat_worst(cap, jt);
-    int T = 32;
-    {   // threads per instance: the big systems are latency bound -> many warps per instance
-        size_t d = 2 * (size_t)cap;
-        T = d <= 64 ? 32 : (d <= 128 ? 128 : (d <= 256 ? 256 : 512));
-    }
+    int T = pivot_threads(2 * (size_t)cap);
     if (fixed + want > (size_t)h->max_smem_optin) {
         // does not fit with the worst case: clipped matrix (the kernel checks the ACTUAL system of every instance against it)
-        if (T == 32) { T = 128; }
         if (fixed + 1024 > (size_t)h->max_smem_optin) return fail(B200PF_E_CAPACITY, "grid too large for the on-chip workspace");
         size_t avail = ((size_t)h->max_smem_optin - fixed) & ~size_t(15);
         if (want > avail) want = avail;
@@ -793,30 +811,6 @@ static int generic_config(b200pf_handle *h, int cap, int jt, int *T_out, size_t 
 // Safety net of a planned launch (b200pf_redo.cuh): the configuration of the pivoting re-solve the planned kernel tail-launches
 // when one of its instances ends as ST_DIV (RedoDesc).  fp64 Jacobian whenever the actual systems fit the workspace with it
 // (5 / 14 / 36 substations), in global memory otherwise (118 substations).
-template <int T>
-static int redo_smem(b200pf_handle *h, const RedoDesc &rd, int *smem_out) {
-    const DevGrid &g = h->g;
-    // (matrix in global memory: the shared-memory workspace only holds the bus arrays)
-    WsLayout L = ws_layout(rd.nb_cap, g.n_slot, g.n_line, g.n_inj, rd.mat ? (size_t)16 : (size_t)rd.mat_bytes);
-    const size_t smem = L.total;
-    if (smem > (size_t)h->max_smem_optin) return fail(B200PF_E_CAPACITY, "workspace does not fit in shared memory");
-    // The attribute holds for launches from the device as well.  It is set only when a launch needs more than any before it
-    // (per device and variant, shared by all handles: a larger limit never hurts): this runs ahead of every planned launch,
-    // and setting the attribute each time kept the GPU waiting for the host between steps.
-    static std::mutex mu;
-    static std::unordered_map<int, int> done;           // device * 1024 + T -> largest limit set
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        int &cur = done[h->device * 1024 + T];
-        if ((int)smem > cur) {
-            CU(cudaFuncSetAttribute(pf_kernel_redo<T, double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            cur = (int)smem;
-        }
-    }
-    *smem_out = (int)smem;
-    return 0;
-}
-
 static int redo_config(b200pf_handle *h, const RunArgs &a, int nb_cap_req, RedoDesc *rd) {
     *rd = RedoDesc{};
     if (!h->redo_enabled || a.is_dc || !a.topo) return 0;     // (the DC solve is a product with the plan's inverse: nothing to pivot)
@@ -848,8 +842,7 @@ static int redo_config(b200pf_handle *h, const RunArgs &a, int nb_cap_req, RedoD
         }
         rd->mat = rs.mat; rd->mat_stride = rs.stride;
         want = worst;
-        const size_t d = 2 * (size_t)cap;
-        T = d <= 64 ? 32 : (d <= 128 ? 128 : (d <= 256 ? 256 : 512));
+        T = pivot_threads(2 * (size_t)cap);
     } else {
         int rc = generic_config(h, cap, 8, &T, &want);
         if (rc) return rc;
@@ -858,13 +851,18 @@ static int redo_config(b200pf_handle *h, const RunArgs &a, int nb_cap_req, RedoD
     rd->grid = (a.batch + 31) / 32;
     if (rd->grid > max_ctas) rd->grid = max_ctas;
     if (rd->grid < 1) rd->grid = 1;
-    int rc;
+    // (matrix in global memory: the shared-memory workspace only holds the bus arrays)
+    WsLayout L = ws_layout(cap, g.n_slot, g.n_line, g.n_inj, rd->mat ? (size_t)16 : want);
+    if (L.total > (size_t)h->max_smem_optin) return fail(B200PF_E_CAPACITY, "workspace does not fit in shared memory");
+    rd->smem = (int)L.total;
+    const void *kern;
     switch (T) {
-        case 32: rc = redo_smem<32>(h, *rd, &rd->smem); break;
-        case 128: rc = redo_smem<128>(h, *rd, &rd->smem); break;
-        case 256: rc = redo_smem<256>(h, *rd, &rd->smem); break;
-        default: rc = redo_smem<512>(h, *rd, &rd->smem); break;
+        case 32: kern = (const void *)pf_kernel_redo<32, double>; break;
+        case 128: kern = (const void *)pf_kernel_redo<128, double>; break;
+        case 256: kern = (const void *)pf_kernel_redo<256, double>; break;
+        default: kern = (const void *)pf_kernel_redo<512, double>; break;
     }
+    int rc = raise_smem_limit(h, kern, rd->smem);
     if (rc) return rc;
     rd->on = 1;
     return 0;
@@ -905,7 +903,6 @@ static int stat_sync(b200pf_handle *h) {
 
 template <int T, int U, int MINB, bool PROT, int WPC = 1, bool STAGE = false, bool UNI = false, int MODE = 0>
 static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel, const RedoDesc &rd) {
-    const DevGrid &g = h->g;
     constexpr int G = T < 32 ? 32 / T : 1;
     constexpr int BLOCK = (T < 32 ? 32 : T) * WPC;
     auto kern = pf_kernel_block<T, U, MINB, PROT, WPC, STAGE, UNI, MODE>;
@@ -921,23 +918,9 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     }
     if (STAGE) { int rc = stat_sync(h); if (rc) return rc; }
     const int smem = ws * WPC + plan_bytes + (STAGE ? h->stat_off.total : 0);
-    const int variant = 1000 + MINB * 4096 + T * 64 + U * 8 + (PROT ? 1 : 0) + (STAGE ? 2 : 0) + (WPC > 1 ? 4 : 0) + (UNI ? 100000 : 0) + MODE * 200000;
-    if (h->sparse_occ_smem != smem || h->sparse_occ_variant != variant) {
-        // (the staged variant owns a few bytes of static shared memory: dynamic + static must stay within the opt-in limit)
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, h->max_smem_optin - 256));
-        int occ = 1;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, BLOCK, (size_t)smem));
-        if (occ < 1) occ = 1;
-        int cap = h->sparse_cta_cap;
-        if (cap == 0 && G == 1 && smem >= 16 * 1024) cap = (164 * 1024) / (smem + 1024);   // large workspaces: leave ~90 KB of L1 for the plan arrays
-        if (cap > 0 && occ > cap) {
-            occ = cap;
-            int pct = (int)(((size_t)occ * (size_t)(smem + 1024) * 100 + (size_t)h->max_smem_optin - 1) / (size_t)h->max_smem_optin);
-            if (pct > 100) pct = 100;
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
-        }
-        h->sparse_occ = occ; h->sparse_occ_smem = smem; h->sparse_occ_variant = variant;
-    }
+    // (the staged variant owns a few bytes of static shared memory: dynamic + static must stay within the opt-in limit)
+    int rc = planned_occupancy(h, (const void *)kern, BLOCK, smem, h->max_smem_optin - 256, G == 1);
+    if (rc) return rc;
     PlanArgs pa{};
     pa.blobs = h->d_plan_blobs;
     pa.plan_off = h->d_plan_off + (sel.d_inst_plan ? 0 : sel.single);
@@ -945,16 +928,9 @@ static int launch_block_t(b200pf_handle *h, const RunArgs &a, const PlanSel &sel
     pa.lay_nb = sel.lay_nb; pa.lay_nblkA = sel.lay_nblkA;
     pa.stat = STAGE ? h->d_stat : nullptr; pa.so = h->stat_off;
     const int n_cta_work = ((a.batch + G - 1) / G + WPC - 1) / WPC;
-    const int resident = h->sm_count * h->sparse_occ;
-    const int rounds = (n_cta_work + resident - 1) / resident;
-    int grid = (n_cta_work + rounds - 1) / rounds;
-    if (grid < 1) grid = 1;
-    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(g, a, pa, ws, plan_bytes, plan_src, row_ahead, rd);
-    CU(cudaGetLastError());
-    h->launches++;
-    h->last_smem = smem; h->last_T = T; h->last_grid = grid; h->last_block = BLOCK; h->last_kernel = 4;
-    set_last_cfg(h, {T, U, MINB, PROT ? 1 : 0, WPC, STAGE ? 1 : 0, UNI ? 1 : 0, MODE});
-    return 0;
+    const int grid = balanced_grid(n_cta_work, h->sm_count * h->sparse_occ);
+    kern<<<grid, BLOCK, (size_t)smem, h->stream>>>(h->g, a, pa, ws, plan_bytes, plan_src, row_ahead, rd);
+    return launched(h, KERN_PLANNED_BLOCK, smem, T, grid, BLOCK, {T, U, MINB, PROT ? 1 : 0, WPC, STAGE ? 1 : 0, UNI ? 1 : 0, MODE});
 }
 
 // compiled (lanes, operations per lane and row) variants; U > 1 and 2 lanes per instance were slower in variant sweeps
@@ -1012,39 +988,22 @@ static int launch(b200pf_handle *h, RunArgs a, int nb_cap_req, const PlanSel *se
         return rc ? rc : launch_sparse(h, a, *sel, rd);
     }
     const DevGrid &g = h->g;
-    if (h->env_flags < 0) {
-        const char *f64 = getenv("B200PF_JACOBIAN_FP64"), *nosk = getenv("B200PF_NO_SMALL_KERNEL");
-        h->env_flags = ((f64 && f64[0] == '1') ? 1 : 0) | ((nosk && nosk[0] == '1') ? 2 : 0);
-    }
-    const bool jd = (h->env_flags & 1) != 0;
-    const int jt = jd ? 8 : 4;
     int cap = nb_cap_req;
     if (cap <= 0 || cap > g.n_slot) cap = g.n_slot;
-    // warp-per-instance fast path: every element class fits one warp and the caller bounds the number
-    // of active buses so that the Newton system has <= 32 unknowns (see b200pf_small.cuh)
-    if (!jd && !(h->env_flags & 2) && g.n_slot <= 32 && g.n_line <= 32 && g.n_unit <= 32 && g.n_load <= 32 &&
-        g.n_sto <= 32 && g.n_shunt <= 32 && cap <= 17)
-        return launch_small(h, a, cap);
+    // (no bound from the caller is every slot: a grid of at most 17 bus slots takes the warp kernel without one)
+    if (warp_kernel_fits(g, cap)) return launch_small(h, a, cap);
     if (a.prot) return fail(B200PF_E_STATE, "device-side protections need the warp-per-instance kernel (<= 32 lines / bus slots, nb_cap <= 17)");
     int T = 32;
     size_t want = 0;
-    int rc = generic_config(h, cap, jt, &T, &want);
+    int rc = generic_config(h, cap, 4, &T, &want);
     if (rc) return rc;
     a.nb_cap = cap;
     a.mat_bytes = (int)want;
-    if (jd) {
-        switch (T) {
-            case 32: return launch_t<32, double>(h, a);
-            case 128: return launch_t<128, double>(h, a);
-            case 256: return launch_t<256, double>(h, a);
-            default: return launch_t<512, double>(h, a);
-        }
-    }
     switch (T) {
-        case 32: return launch_t<32, float>(h, a);
-        case 128: return launch_t<128, float>(h, a);
-        case 256: return launch_t<256, float>(h, a);
-        default: return launch_t<512, float>(h, a);
+        case 32: return launch_t<32>(h, a);
+        case 128: return launch_t<128>(h, a);
+        case 256: return launch_t<256>(h, a);
+        default: return launch_t<512>(h, a);
     }
 }
 
@@ -1074,7 +1033,7 @@ static int run_staged_device(b200pf_handle *h, int batch, int is_dc, int max_ite
     a.topo = h->d_topo; a.inj = h->d_inj; a.out = h->d_out; a.status = h->d_status; a.iters = h->d_iters;
     a.busv = want_busv ? h->d_busv : nullptr;
     PlanSel sel;
-    const int use = plan_select(h, h->h_topo, batch, 0, 0, h->stream, &sel, nb_cap);
+    const int use = plan_select(h, h->h_topo, batch, 0, 0, h->stream, &sel);
     if (use < 0) return use;
     return launch(h, a, nb_cap, use ? &sel : nullptr);
 }
@@ -1088,7 +1047,7 @@ extern "C" int b200pf_run_device_topo(b200pf_handle *h, int batch, const int8_t 
     RunArgs a = base_args(h, batch, is_dc, max_iter, tol_mva);
     a.topo = d_topo; a.inj = d_inj; a.out = d_out; a.status = d_status; a.iters = d_iters; a.busv = d_busv;
     PlanSel sel;
-    const int use = plan_select(h, host_topo, batch, 0, 0, h->stream, &sel, nb_cap);
+    const int use = plan_select(h, host_topo, batch, 0, 0, h->stream, &sel);
     if (use < 0) return use;
     return launch(h, a, nb_cap, use ? &sel : nullptr);
 }
@@ -1177,7 +1136,7 @@ static int series_plans(b200pf_handle *h, const int8_t *topo) {
     h->series_plans_stale = false;
     PlanSel sel;
     CU(cudaStreamSynchronize(h->stream));
-    const int use = plan_select(h, topo, h->series_batch, 0, 0, h->stream, &sel, -1);
+    const int use = plan_select(h, topo, h->series_batch, 0, 0, h->stream, &sel);
     if (use < 0) return use;
     if (!use) return 0;
     h->series_plan_single = sel.single; h->series_plan_smem = sel.smem; h->series_lay_nb = sel.lay_nb; h->series_lay_nblkA = sel.lay_nblkA;
@@ -1223,9 +1182,8 @@ static int series_step_planned_prot(b200pf_handle *h, RunArgs a) {
         PlanSel sel;
         sel.single = 0; sel.d_inst_plan = h->d_series_plan;
         sel_layout(h, &sel, false);
-        RedoDesc rd;       // (the re-solve applies the protection rules to what it solves)
-        int rc = redo_config(h, a, 0, &rd);
-        if (rc || (rc = launch_sparse(h, a, sel, rd))) return rc;
+        int rc = launch(h, a, 0, &sel);      // (the re-solve applies the protection rules to what it solves)
+        if (rc) return rc;
         int nflag = 0;
         CU(cudaMemcpyAsync(&nflag, h->d_nflag, 4, cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));
@@ -1291,15 +1249,15 @@ static int series_step_impl(b200pf_handle *h, int is_dc, int max_iter, double to
         a.pcount = h->d_pcount; a.ts_over = h->d_tsover; a.disc = h->d_disc; a.done = h->d_done;
     }
     h->next_reset = 0;
+    // the warp kernel runs the series' protections only under a bound from the caller (nb_cap > 0), although launch() reads
+    // nb_cap <= 0 as every slot and so takes the warp kernel without one on a grid of at most 17 bus slots
+    const bool small_ok = nb_cap > 0 && warp_kernel_fits(h->g, nb_cap);
     if (h->series_dev_topo_ahead && h->plan_policy != 1) {
         // protections ran on the device (warp kernel: trips written into d_series_topo); whoever uses plans next — protections
         // switched off, policy switched to the planned kernel — must see those outages: refresh the host mirror and the plans
-        const DevGrid &gg = h->g;
-        const bool small_ok = gg.n_slot <= 32 && gg.n_line <= 32 && gg.n_unit <= 32 && gg.n_load <= 32 && gg.n_sto <= 32 && gg.n_shunt <= 32 &&
-                              nb_cap > 0 && nb_cap <= 17;
         const bool warp_again = h->prot && small_ok && h->plan_policy != 2 && !is_dc;
         if (!warp_again) {
-            std::vector<int8_t> cur((size_t)h->series_batch * gg.n_topo_in);
+            std::vector<int8_t> cur((size_t)h->series_batch * h->g.n_topo_in);
             CU(cudaStreamSynchronize(h->stream));
             CU(cudaMemcpy(cur.data(), h->d_series_topo, cur.size(), cudaMemcpyDeviceToHost));
             int rc = series_plans(h, cur.data());
@@ -1313,15 +1271,10 @@ static int series_step_impl(b200pf_handle *h, int is_dc, int max_iter, double to
         int rc = series_plans(h, keep.data());
         if (rc) return rc;
     }
-    {
-        const DevGrid &gg = h->g;
-        const bool small_ok = gg.n_slot <= 32 && gg.n_line <= 32 && gg.n_unit <= 32 && gg.n_load <= 32 && gg.n_sto <= 32 && gg.n_shunt <= 32 &&
-                              nb_cap > 0 && nb_cap <= 17;
-        // protections: the warp kernel cascades entirely on the device (no host in the loop) and is preferred where it applies;
-        // everything else runs the planned kernel with the host re-planning the instances whose lines trip
-        if (h->prot && h->series_plan_state && h->plan_policy != 1 && (h->plan_policy == 2 || !small_ok) && !is_dc)
-            return series_step_planned_prot(h, a);
-    }
+    // protections: the warp kernel cascades entirely on the device (no host in the loop) and is preferred where it applies;
+    // everything else runs the planned kernel with the host re-planning the instances whose lines trip
+    if (h->prot && h->series_plan_state && h->plan_policy != 1 && (h->plan_policy == 2 || !small_ok) && !is_dc)
+        return series_step_planned_prot(h, a);
     if (h->series_plan_state && !h->prot && h->plan_policy != 1) {
         PlanSel sel;
         sel.single = h->series_plan_single; sel.smem = h->series_plan_smem; sel.lay_nb = h->series_lay_nb; sel.lay_nblkA = h->series_lay_nblkA;
@@ -1473,7 +1426,7 @@ extern "C" int b200pf_n1_host(b200pf_handle *h, int batch, const int8_t *topo, c
     a.topo = h->d_topo; a.inj = h->d_inj; a.out = nullptr; a.status = h->d_status; a.iters = h->d_iters; a.busv = nullptr;
     a.n1_lines = g.n_line; a.th_lim = h->d_thlim; a.rho = h->d_rho;
     PlanSel sel;
-    const int use = plan_select(h, topo, batch, g.n_line, 0, h->stream, &sel, nb_cap);
+    const int use = plan_select(h, topo, batch, g.n_line, 0, h->stream, &sel);
     if (use < 0) return use;
     int rc = launch(h, a, nb_cap, use ? &sel : nullptr);
     if (rc) return rc;
@@ -1509,7 +1462,7 @@ extern "C" int b200pf_run_rows_staged(b200pf_handle *h, int batch, int is_dc, in
     a.topo = h->d_topo; a.inj = nullptr; a.out = h->d_out; a.status = h->d_status; a.iters = h->d_iters; a.busv = nullptr;
     a.series = 1; a.rows = h->d_rows; a.static_inj = h->d_static_inj;
     PlanSel sel;
-    const int use = plan_select(h, h->h_topo, batch, 0, 0, h->stream, &sel, nb_cap);
+    const int use = plan_select(h, h->h_topo, batch, 0, 0, h->stream, &sel);
     if (use < 0) return use;
     int rc = launch(h, a, nb_cap, use ? &sel : nullptr);
     if (rc) return rc;
@@ -1565,7 +1518,7 @@ static int rows_chunk_launch_impl(b200pf_handle *h, int first, int count, const 
     }
     const size_t F = (size_t)first, C = (size_t)count, ncol = 2 * (size_t)g.n_load + 2 * (size_t)g.n_gen;
     PlanSel sel;
-    const int use = plan_select(h, h->h_topo + F * g.n_topo_in, count, 0, first, st, &sel, nb_cap);
+    const int use = plan_select(h, h->h_topo + F * g.n_topo_in, count, 0, first, st, &sel);
     if (use < 0) return use;
     RunArgs a = base_args(h, count, is_dc, max_iter, tol_mva);
     a.topo = h->d_topo + F * g.n_topo_in; a.inj = nullptr; a.out = h->d_out + F * g.n_out; a.status = h->d_status + F;
