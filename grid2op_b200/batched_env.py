@@ -114,6 +114,7 @@ class BatchedEnv(BatchedDoNothing):
         self._authority = "host"
         self._opp = None                                                   # line-attack opponent (:meth:`enable_opponent`)
         self._alerts = None                                                # line alerts (:meth:`enable_alerts`)
+        self._alarms = None                                                # alarms (:meth:`enable_alarms`)
 
     # ------------------------------------------------------------------------------------------------------------
     def _bus_cap(self) -> int:
@@ -268,11 +269,13 @@ class BatchedEnv(BatchedDoNothing):
                 self._topo_dirty = True
                 self._cap_dirty[ii[was_on]] = True
 
-    def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None):
+    def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
+             raise_alarm=None):
         """One env.step of every instance.  ``sub_id`` int [B] (-1: none) with ``sub_bus`` int8 [B, >= max_sub_size] (busbar per
         element of that substation in topology-vector order, 0 = leave); ``line_id`` int [B] (-1: none) with ``line_status``
         int [B] (+1 reconnect / -1 disconnect); ``raise_alert`` bool [B, dim_alerts] (:meth:`enable_alerts`; None: no alert,
-        ignored on a reset step).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the device (:meth:`fetch`)."""
+        ignored on a reset step); ``raise_alarm`` bool [B, dim_alarms] (:meth:`enable_alarms`; None: no alarm, ignored on a reset
+        step).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the device (:meth:`fetch`)."""
         if raise_alert is not None:
             if self._alerts is None:
                 raise ValueError("raise_alert without enable_alerts()")
@@ -280,6 +283,13 @@ class BatchedEnv(BatchedDoNothing):
             if raise_alert.shape != (self.batch, self._alerts.n) or raise_alert.dtype.kind not in "bui":
                 raise ValueError(f"raise_alert must be a bool array of shape {(self.batch, self._alerts.n)}")
             raise_alert = raise_alert != 0
+        if raise_alarm is not None:
+            if self._alarms is None:
+                raise ValueError("raise_alarm without enable_alarms()")
+            raise_alarm = np.asarray(raise_alarm)
+            if raise_alarm.shape != (self.batch, self._alarms.n) or raise_alarm.dtype.kind not in "bui":
+                raise ValueError(f"raise_alarm must be a bool array of shape {(self.batch, self._alarms.n)}")
+            raise_alarm = raise_alarm != 0
         self._to_host()
         gm = self.gm
         opp = None
@@ -350,11 +360,19 @@ class BatchedEnv(BatchedDoNothing):
                 self._obs["reset"][live] = True
         else:
             self.current_step[live] += 1
+        alarm_reward = None
+        if self._alarms is not None:          # registered once the step's legality is known; an instance finished before keeps its state
+            alarm_reward = self._alarms.step(None if from_reset else raise_alarm, live & (not from_reset), self.is_illegal,
+                                             self.current_step, newly_done, disc).copy()
         info = {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done, "is_illegal": self.is_illegal.copy()}
         if opp is not None:
             info["opponent_attack_line"], info["opponent_attack_duration"] = opp
         if alert_reward is not None and self._alerts.reward:
             info["rewards"] = {"alert": alert_reward}
+        if alarm_reward is not None:
+            info["is_alarm_illegal"] = self._alarms.s["illegal"].astype(bool)
+            if self._alarms.reward:
+                info["rewards"] = {"alarm": alarm_reward}
         return rho, self.done.copy(), info
 
     # ---- line alerts ------------------------------------------------------------------------------------------------------
@@ -372,6 +390,8 @@ class BatchedEnv(BatchedDoNothing):
         from .alert import BatchedAlerts
         if self._obs is not None:
             raise RuntimeError("enable_alerts() before enable_observation(): the observation width depends on dim_alerts")
+        if self._alarms is not None:
+            raise ValueError("alerts and alarms are exclusive (an environment's alerts_info.json has \"by_line\" or \"fixed\")")
         names = list(getattr(self.gm, "name_line", []))
         flat = []
         for x in alertable_lines:
@@ -409,6 +429,53 @@ class BatchedEnv(BatchedDoNothing):
             raise RuntimeError("call enable_alerts() first")
         self._to_host()
         return self._alerts.get_state()
+
+    # ---- alarms -----------------------------------------------------------------------------------------------------------
+    def enable_alarms(self, zones, *, max_budget: float = 3.0, budget_per_ts: float = 1.0 / 192, alarm_cost: float = 1.0,
+                      init_budget: float = 2.0, alarm_best_time: int = 12, alarm_window_size: int = 12, reward: bool = True):
+        """grid2op's alarms (l2rpn_icaps_2021) for every instance: ``zones`` the ``(names, zone mask per line)`` pair
+        :func:`grid2op_b200.alarm.load_alarm_zones` reads from the environment's ``alerts_info.json``; the
+        ``LinearAttentionBudget`` constants of the environment's ``kwargs_attention_budget``; ``alarm_best_time`` /
+        ``alarm_window_size``: the ``ALARM_BEST_TIME`` / ``ALARM_WINDOW_SIZE`` parameters; ``reward``: compute ``AlarmReward`` into
+        ``info["rewards"]["alarm"]`` (float64 [B], 0 for an instance finished before the step, non-zero only on the step that ends
+        an episode).  From then on :meth:`step` / :meth:`step_tensors` take ``raise_alarm``, ``info["is_alarm_illegal"]`` (bool [B])
+        says which alarms the budget refused, and :meth:`observe` fills the five alarm attributes.  Call it before
+        :meth:`enable_observation` (the vector's width depends on ``dim_alarms``).  Alarms and alerts are exclusive; a ring of
+        ``alarm_best_time + alarm_window_size`` steps is kept per instance, at most 1024.  AlarmReward's ``reward_max`` at the end
+        of the chronics is never paid: this environment has no end of chronics, the caller resets."""
+        from .alarm import MAX_RING, MAX_ZONES, BatchedAlarms
+        if self._obs is not None:
+            raise RuntimeError("enable_alarms() before enable_observation(): the observation width depends on dim_alarms")
+        if self._alerts is not None:
+            raise ValueError("alerts and alarms are exclusive (an environment's alerts_info.json has \"by_line\" or \"fixed\")")
+        names, mask = zones
+        mask = np.asarray(mask)
+        n = len(names)
+        if not 1 <= n <= MAX_ZONES:
+            raise ValueError(f"{n} alarm zones, 1 to {MAX_ZONES} supported")
+        if mask.shape != (self.gm.n_line,) or mask.dtype.kind not in "ui" or (mask <= 0).any() or (mask >= 2 ** n).any():
+            raise ValueError(f"the zone masks must be {self.gm.n_line} integers, each line in at least one of the {n} zones")
+        best, win = int(alarm_best_time), int(alarm_window_size)
+        if best <= 0 or win <= 0:
+            raise ValueError("alarm_best_time and alarm_window_size must be >= 1")
+        if best + win > MAX_RING:
+            raise ValueError(f"alarm_best_time + alarm_window_size must be <= {MAX_RING}")
+        self._to_host()
+        self._alarms = BatchedAlarms(mask, n, self.batch, max_budget=max_budget, budget_per_ts=budget_per_ts, alarm_cost=alarm_cost,
+                                     init_budget=init_budget, best_time=best, window_size=win, reward=reward)
+        self._alarms.names = list(names)
+        if self._dev is not None:
+            self._alarm_bind_device()
+        return n
+
+    def alarm_state(self) -> dict:
+        """the alarm state of every instance as the device keeps it (:data:`grid2op_b200.alarm.ALARM_STATE`): budget float32 [B];
+        time_last, time_last_ok int32 [B]; last, last_ok int32 [B, n_zone]; the ring of successful alarms ring_step int32 /
+        ring_mask uint32 [B, best_time + window_size]; any_ok, used (AlarmReward.is_alarm_used), illegal uint8 [B]"""
+        if self._alarms is None:
+            raise RuntimeError("call enable_alarms() first")
+        self._to_host()
+        return self._alarms.get_state()
 
     # ---- line-attack opponent ---------------------------------------------------------------------------------------------
     def enable_opponent(self, kind: str, lines_attacked, *, attack_duration: int, attack_cooldown: int, budget_per_ts: float,
@@ -558,6 +625,8 @@ class BatchedEnv(BatchedDoNothing):
             self._opp.reset(idx)
         if self._alerts is not None:
             self._alerts.reset(idx)
+        if self._alarms is not None:
+            self._alarms.reset(idx)
         self.engine.series_reset_instances(idx, t_new=rows % self.chron.shape[1], topo_rows=self.topo[idx])
         self._cap_dirty[idx] = True
         if self.tight_cap:
@@ -577,7 +646,8 @@ class BatchedEnv(BatchedDoNothing):
             raise ValueError(f"unknown reward class {reward!r} (RedispReward, L2RPNReward or None)")
         gm = self.gm
         n_alert = self._alerts.n if self._alerts is not None else 0
-        seg, n_obs = ob.obs_spec(gm, attrs, n_alert)
+        n_alarm = self._alarms.n if self._alarms is not None else 0
+        seg, n_obs = ob.obs_spec(gm, attrs, n_alert, n_alarm)
         folders = list(scenarios) if scenarios is not None else list_scenarios(os.path.join(env_dir, "chronics"))
         if len(folders) != self.chron.shape[0]:
             raise ValueError(f"{len(folders)} scenario folders for {self.chron.shape[0]} scenarios of the chronics array")
@@ -590,18 +660,20 @@ class BatchedEnv(BatchedDoNothing):
                  maint_time=self._maint_time, maint_dur=self._maint_dur, reward_kind=ob.REWARDS[reward],
                  reward=ob.reward_constants(gen, dt_min) if gen["available"] else dict(max_regret=0.0, reward_min=0.0, reward_illegal=0.0,
                                                                                        dts_hours=dt_min / 60.0),
-                 soft_thr=self.soft_overflow_threshold, n_alert=n_alert)
+                 soft_thr=self.soft_overflow_threshold, n_alert=n_alert, n_alarm=n_alarm)
         if reward == "L2RPNReward":
             t["reward"]["reward_min"] = 0.0
         self.engine.obs_bind(t)
         self._obs = dict(tables=t, n_obs=n_obs, reward=reward, reset=np.ones(self.batch, dtype=bool),
-                         host_in=np.zeros((self.batch, gm.n_line + gm.n_sub + 3 + (6 * n_alert + 1 if n_alert else 0)), dtype=np.int32))
+                         host_in=np.zeros((self.batch, gm.n_line + gm.n_sub + 3 + (6 * n_alert + 1 if n_alert else 0) +
+                                           (n_alarm + 4 if n_alarm else 0)), dtype=np.int32))
         return n_obs
 
     def observe_inputs(self) -> np.ndarray:
         """int32 [B, n_line + n_sub + 3]: the per-instance values only the host knows (cooldowns, current_step, step stamp, flags
         illegal / game over / reset) — what one observe launch copies to the device; with alerts, 6 dim_alerts + 1 more columns
-        (the alert values, :meth:`grid2op_b200.alert.BatchedAlerts.obs_record`)."""
+        (the alert values, :meth:`grid2op_b200.alert.BatchedAlerts.obs_record`); with alarms, dim_alarms + 4 more (the alarm values,
+        :meth:`grid2op_b200.alarm.BatchedAlarms.obs_record`)."""
         self._to_host()
         gm, o = self.gm, self._obs
         h = o["host_in"]
@@ -610,7 +682,9 @@ class BatchedEnv(BatchedDoNothing):
         h[:, nl + ns] = self.current_step; h[:, nl + ns + 1] = self.n_steps
         h[:, nl + ns + 2] = self.is_illegal * 1 + self.done * 2 + o["reset"] * 4
         if self._alerts is not None:
-            h[:, nl + ns + 3:] = self._alerts.obs_record()
+            h[:, nl + ns + 3:nl + ns + 4 + 6 * self._alerts.n] = self._alerts.obs_record()
+        if self._alarms is not None:
+            h[:, h.shape[1] - self._alarms.n - 4:] = self._alarms.obs_record(self.current_step)
         return h
 
     def observe(self, obs_out=None, reward_out=None):
@@ -698,6 +772,8 @@ class BatchedEnv(BatchedDoNothing):
             self._opp_bind_device()
         if self._alerts is not None:
             self._alert_bind_device()
+        if self._alarms is not None:
+            self._alarm_bind_device()
         return st
 
     def _opp_bind_device(self):
@@ -734,6 +810,16 @@ class BatchedEnv(BatchedDoNothing):
         self.engine.alert_bind(a, d["alert_raise"].data_ptr(), d["alert_reward"].data_ptr())
         self._authority = "host"              # (the next step_tensors pushes the whole state, the alerts' included)
 
+    def _alarm_bind_device(self):
+        """the alarm constants to the device; the step's raise_alarm, AlarmReward and is_alarm_illegal are device buffers of ours"""
+        import torch
+        d, a, B = self._dev, self._alarms, self.batch
+        d["alarm_raise"] = torch.zeros((B, a.n), dtype=torch.uint8, device=d["device"])
+        d["alarm_reward"] = torch.zeros(B, dtype=torch.float64, device=d["device"])
+        d["alarm_illegal"] = torch.zeros(B, dtype=torch.bool, device=d["device"])        # (written as uint8 0 / 1)
+        self.engine.alarm_bind(a, d["alarm_raise"].data_ptr(), d["alarm_reward"].data_ptr(), d["alarm_illegal"].data_ptr())
+        self._authority = "host"              # (the next step_tensors pushes the whole state, the alarms' included)
+
     def _to_device(self):
         """hand the host state to the tensor path"""
         import torch
@@ -756,6 +842,8 @@ class BatchedEnv(BatchedDoNothing):
                 self.engine.opp_multi_set_state(s)
         if self._alerts is not None:
             self.engine.alert_set_state(self._alerts.get_state())
+        if self._alarms is not None:
+            self.engine.alarm_set_state(self._alarms.get_state())
         self._illegal_seen = self.engine.env_stats()["n_illegal"]
         self._authority = "device"
 
@@ -784,10 +872,14 @@ class BatchedEnv(BatchedDoNothing):
         if self._alerts is not None:
             self._alerts.set_state(self.engine.alert_get_state())
             self._alerts.reward_out[:] = self._dev["alert_reward"].cpu().numpy()
+        if self._alarms is not None:
+            self._alarms.set_state(self.engine.alarm_get_state())
+            self._alarms.reward_out[:] = self._dev["alarm_reward"].cpu().numpy()
         if self.tight_cap and self._cap_dirty.any():
             self.nb_cap = self._bus_cap()
 
-    def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None):
+    def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
+                     raise_alarm=None):
         """:meth:`step` with the actions as CUDA tensors and the state kept on the device: ``sub_id`` int32 / int64 [B] (-1: none)
         with ``sub_bus`` int8 / int32 / int64 [B, >= max_sub_size]; ``line_id`` int32 / int64 [B] (-1: none) with ``line_status``
         int32 / int64 [B] (> 0 reconnect / < 0 disconnect).  Same semantics and bit-identical state as :meth:`step`; ordered against torch's current
@@ -796,7 +888,9 @@ class BatchedEnv(BatchedDoNothing):
         are the environment's own buffers: the next step overwrites them.  The host waits once per step for a few words (and
         copies back the changed topology rows when the plans have to be looked up, which waits again).  An id or busbar out of
         range raises ValueError and changes nothing.  ``raise_alert``: bool / uint8 CUDA tensor [B, dim_alerts] (:meth:`enable_alerts`;
-        None: no alert); ``info["rewards"]["alert"]`` is then the environment's float64 [B] buffer of the AlertReward."""
+        None: no alert); ``info["rewards"]["alert"]`` is then the environment's float64 [B] buffer of the AlertReward.
+        ``raise_alarm``: bool / uint8 CUDA tensor [B, dim_alarms] (:meth:`enable_alarms`; None: no alarm); ``info["rewards"]["alarm"]``
+        and ``info["is_alarm_illegal"]`` are then the environment's float64 / bool [B] buffers."""
         import torch
         d = self._tensor_state()
         dev, B = d["device"], self.batch
@@ -831,6 +925,10 @@ class BatchedEnv(BatchedDoNothing):
             if self._alerts is None:
                 raise ValueError("raise_alert without enable_alerts()")
             _check_tensor(raise_alert, "raise_alert", (B, self._alerts.n), (torch.bool, torch.uint8), dev)
+        if raise_alarm is not None:
+            if self._alarms is None:
+                raise ValueError("raise_alarm without enable_alarms()")
+            _check_tensor(raise_alarm, "raise_alarm", (B, self._alarms.n), (torch.bool, torch.uint8), dev)
         if self._authority != "device":
             self._to_device()
         if self._alerts is not None:                      # (on torch's stream: ordered before the engine's launches below)
@@ -838,6 +936,11 @@ class BatchedEnv(BatchedDoNothing):
                 d["alert_raise"].zero_()
             else:
                 d["alert_raise"].copy_(raise_alert != 0)
+        if self._alarms is not None:
+            if raise_alarm is None:
+                d["alarm_raise"].zero_()
+            else:
+                d["alarm_raise"].copy_(raise_alarm != 0)
         cur, eng = self._streams()
         eng.wait_stream(cur)
         try:
@@ -862,6 +965,10 @@ class BatchedEnv(BatchedDoNothing):
             info["opponent_attack_duration"] = d["opp_dur"]
         if self._alerts is not None and self._alerts.reward:
             info["rewards"] = {"alert": d["alert_reward"]}
+        if self._alarms is not None:
+            info["is_alarm_illegal"] = d["alarm_illegal"]
+            if self._alarms.reward:
+                info["rewards"] = {"alarm": d["alarm_reward"]}
         return d["rho"], d["done"], info
 
     def _reset_tensors(self, mask, rows=None):

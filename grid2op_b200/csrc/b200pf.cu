@@ -132,6 +132,9 @@ struct b200pf_handle {
     // line alerts of the device environment (b200pf_alert_bind)
     AlertArgs alert{}; int alert_batch = 0;
     std::vector<void *> alert_allocs;
+    // alarms of the device environment (b200pf_alarm_bind)
+    AlarmArgs alarm{}; int alarm_batch = 0;
+    std::vector<void *> alarm_allocs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -344,6 +347,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     if (h->h_env_ctl) cudaFreeHost(h->h_env_ctl);
     for (void *p : h->opp_allocs) cudaFree(p);
     for (void *p : h->alert_allocs) cudaFree(p);
+    for (void *p : h->alarm_allocs) cudaFree(p);
     delete h;
     return 0;
 }
@@ -1695,6 +1699,7 @@ extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
     if (g.n_sto && (!d->sto_charge0 || !d->sto_loss_step)) return fail(B200PF_E_ARG, "storage tables missing");
     if (d->reward_kind < B200PF_REWARD_NONE || d->reward_kind > B200PF_REWARD_L2RPN) return fail(B200PF_E_ARG, "unknown reward kind");
     if (d->n_alert < 0 || d->n_alert > ALERT_MAX_LINES) return fail(B200PF_E_ARG, "n_alert out of range");
+    if (d->n_alarm < 0 || d->n_alarm > ALARM_MAX_ZONES) return fail(B200PF_E_ARG, "n_alarm out of range");
     for (int s = 0; s < d->n_seg; ++s)
         if (d->seg[3 * s] < 0 || d->seg[3 * s] >= OS_N_SOURCES || d->seg[3 * s + 1] < 0 || d->seg[3 * s + 2] < 0 ||
             d->seg[3 * s + 1] + d->seg[3 * s + 2] > d->n_obs) return fail(B200PF_E_ARG, "observation segment out of range");
@@ -1740,8 +1745,8 @@ extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
     a.n_seg = d->n_seg; a.n_obs = d->n_obs; a.delta_time = d->delta_time; a.redisp_available = d->redisp_available;
     a.reward_kind = d->reward_kind; a.max_regret = d->max_regret; a.reward_min = d->reward_min; a.reward_illegal = d->reward_illegal;
     a.dts_hours = d->dts_hours; a.soft_thr = d->soft_thr;
-    a.n_alert = d->n_alert;
-    a.host_stride = g.n_line + g.n_sub + 3 + (d->n_alert ? 6 * d->n_alert + 1 : 0);
+    a.n_alert = d->n_alert; a.n_alarm = d->n_alarm;
+    a.host_stride = g.n_line + g.n_sub + 3 + (d->n_alert ? 6 * d->n_alert + 1 : 0) + (d->n_alarm ? d->n_alarm + 4 : 0);
     if (cudaMallocHost(&h->h_obs_in, B * a.host_stride * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
     void *din = nullptr;
     if ((rc = zeros(B * a.host_stride * 4, 0, &din))) return rc;
@@ -1917,14 +1922,22 @@ static AlertArgs env_alert(const b200pf_handle *h) {
     return al;
 }
 
+// the alarms the env launches run (n = 0: none)
+static AlarmArgs env_alarm(const b200pf_handle *h) {
+    if (!h->alarm_batch || h->alarm_batch != h->env_batch) return AlarmArgs{};
+    return h->alarm;
+}
+
 // the observe input record the env launches write: NULL when the observation layer is not bound to this series; an error
-// when its alert values do not match the bound alerts
-static int env_obs_record(const b200pf_handle *h, const AlertArgs &al, int32_t **rec, int *stride) {
+// when its alert or alarm values do not match the bound alerts or alarms
+static int env_obs_record(const b200pf_handle *h, const AlertArgs &al, const AlarmArgs &am, int32_t **rec, int *stride) {
     const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
     *rec = obs ? h->d_obs_in : nullptr;
     *stride = obs ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3;
     if (obs && h->obs.n_alert != al.n)
         return fail(B200PF_E_STATE, "the observation layer and the line alerts disagree on dim_alerts (b200pf_obs_bind / b200pf_alert_bind)");
+    if (obs && h->obs.n_alarm != am.n)
+        return fail(B200PF_E_STATE, "the observation layer and the alarms disagree on dim_alarms (b200pf_obs_bind / b200pf_alarm_bind)");
     return 0;
 }
 
@@ -1947,8 +1960,9 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
         return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
     const AlertArgs al = env_alert(h);
+    const AlarmArgs am = env_alarm(h);
     int32_t *obs_rec; int obs_stride;
-    if (int rc0 = env_obs_record(h, al, &obs_rec, &obs_stride)) return rc0;
+    if (int rc0 = env_obs_record(h, al, am, &obs_rec, &obs_stride)) return rc0;
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2010,7 +2024,7 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     a.status = h->x_status ? h->x_status : h->d_status;
     a.disc = h->prot ? h->d_disc : nullptr;
     a.obs_in = obs_rec; a.obs_stride = obs_stride; a.stamp = stamp;
-    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, al);
+    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, al, am);
     CU(cudaGetLastError());
     h->env_steps++;
     return 0;
@@ -2024,8 +2038,9 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
         return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     const AlertArgs al = env_alert(h);
+    const AlarmArgs am = env_alarm(h);
     int32_t *obs_rec; int obs_stride;
-    if (int rc0 = env_obs_record(h, al, &obs_rec, &obs_stride)) return rc0;
+    if (int rc0 = env_obs_record(h, al, am, &obs_rec, &obs_stride)) return rc0;
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2033,7 +2048,7 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     EnvArgs a = h->env;
     a.reset_mask = d_mask; a.reset_rows = d_rows;
     a.obs_in = obs_rec; a.obs_stride = obs_stride;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi, al);
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi, al, am);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2471,6 +2486,102 @@ extern "C" int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_aler
     const void *src[ALERT_N_BUF] = {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack, launched,
                                     current, cur_id};
     for (int k = 0; k < ALERT_N_BUF; ++k)
+        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
+    CU(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// the alarm state buffers in the order of b200pf_alarm_get_state / _set_state (the last one, is_alarm_illegal, is the caller's),
+// and their bytes for a batch of B
+enum { ALARM_N_BUF = 10 };
+static void alarm_buffers(const AlarmArgs &am, void *p[ALARM_N_BUF]) {
+    void *q[ALARM_N_BUF] = {am.budget, am.time_last, am.time_last_ok, am.last, am.last_ok, am.ring_step, am.ring_mask, am.any_ok,
+                            am.used, am.illegal};
+    for (int k = 0; k < ALARM_N_BUF; ++k) p[k] = q[k];
+}
+static void alarm_sizes(int n, int ring, size_t B, size_t out[ALARM_N_BUF]) {
+    const size_t bn = B * (size_t)n * 4, br = B * (size_t)ring * 4;
+    const size_t s[ALARM_N_BUF] = {B * 4, B * 4, B * 4, bn, bn, br, br, B, B, B};
+    for (int k = 0; k < ALARM_N_BUF; ++k) out[k] = s[k];
+}
+
+extern "C" int b200pf_alarm_bind(b200pf_handle *h, const b200pf_alarm_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    if (d->n_zone < 1 || d->n_zone > ALARM_MAX_ZONES || !d->zone_mask || d->best_time < 1 || d->window_size < 1 ||
+        d->best_time > ALARM_MAX_RING - d->window_size || !d->raise_alarm || !d->reward_out || !d->is_alarm_illegal)
+        return fail(B200PF_E_ARG, "bad alarm description");
+    const uint32_t zones = d->n_zone == 32 ? 0xffffffffu : (1u << d->n_zone) - 1u;
+    for (int l = 0; l < h->g.n_line; ++l)
+        if (!d->zone_mask[l] || (d->zone_mask[l] & ~zones)) return fail(B200PF_E_ARG, "a line in no zone, or in a zone past n_zone");
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (void *p : h->alarm_allocs) cudaFree(p);
+    h->alarm_allocs.clear();
+    h->alarm_batch = 0;
+    const size_t B = (size_t)h->env_batch;
+    AlarmArgs am{};
+    am.n = d->n_zone; am.n_line = h->g.n_line;
+    am.max_budget = d->max_budget; am.budget_per_ts = d->budget_per_ts; am.alarm_cost = d->alarm_cost; am.init_budget = d->init_budget;
+    am.best_time = d->best_time; am.window = d->window_size; am.ring = d->best_time + d->window_size; am.reward = d->reward ? 1 : 0;
+    am.raise = d->raise_alarm; am.reward_out = d->reward_out; am.illegal = d->is_alarm_illegal;
+    void *zm = nullptr;
+    CU(cudaMalloc(&zm, (size_t)am.n_line * 4));
+    h->alarm_allocs.push_back(zm);
+    H2D(zm, d->zone_mask, (size_t)am.n_line * 4);
+    am.zone_mask = (const uint32_t *)zm;
+    size_t sz[ALARM_N_BUF];
+    alarm_sizes(am.n, am.ring, B, sz);
+    void *p[ALARM_N_BUF];
+    for (int k = 0; k < ALARM_N_BUF - 1; ++k) {
+        CU(cudaMalloc(&p[k], sz[k]));
+        h->alarm_allocs.push_back(p[k]);
+    }
+    am.budget = (float *)p[0]; am.time_last = (int32_t *)p[1]; am.time_last_ok = (int32_t *)p[2]; am.last = (int32_t *)p[3];
+    am.last_ok = (int32_t *)p[4]; am.ring_step = (int32_t *)p[5]; am.ring_mask = (uint32_t *)p[6]; am.any_ok = (uint8_t *)p[7];
+    am.used = (uint8_t *)p[8];
+    // every instance starts from LinearAttentionBudget.reset: the initial budget, -1 for the times and zones, an empty ring
+    const std::vector<float> b0(B, d->init_budget);
+    H2D(am.budget, b0.data(), B * 4);
+    for (int k = 1; k < ALARM_N_BUF - 1; ++k) CU(cudaMemsetAsync(p[k], k <= 4 ? 0xff : 0, sz[k], h->stream));
+    CU(cudaMemsetAsync(am.illegal, 0, B, h->stream));
+    CU(cudaMemsetAsync(am.reward_out, 0, B * 8, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->alarm = am; h->alarm_batch = (int)B;
+    return 0;
+}
+
+static bool alarm_bound(const b200pf_handle *h) { return env_bound(h) && h->alarm_batch == h->env_batch; }
+
+extern "C" int b200pf_alarm_get_state(b200pf_handle *h, float *budget, int32_t *time_last, int32_t *time_last_ok, int32_t *last,
+                                      int32_t *last_ok, int32_t *ring_step, uint32_t *ring_mask, uint8_t *any_ok, uint8_t *used,
+                                      uint8_t *illegal) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!alarm_bound(h)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
+    CU(cudaSetDevice(h->device));
+    size_t sz[ALARM_N_BUF];
+    alarm_sizes(h->alarm.n, h->alarm.ring, (size_t)h->alarm_batch, sz);
+    void *src[ALARM_N_BUF];
+    alarm_buffers(h->alarm, src);
+    void *dst[ALARM_N_BUF] = {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal};
+    CU(cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < ALARM_N_BUF; ++k)
+        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
+    return 0;
+}
+
+extern "C" int b200pf_alarm_set_state(b200pf_handle *h, const float *budget, const int32_t *time_last, const int32_t *time_last_ok,
+                                      const int32_t *last, const int32_t *last_ok, const int32_t *ring_step, const uint32_t *ring_mask,
+                                      const uint8_t *any_ok, const uint8_t *used, const uint8_t *illegal) {
+    if (!h) return fail(B200PF_E_ARG, "null handle");
+    if (!alarm_bound(h)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
+    CU(cudaSetDevice(h->device));
+    size_t sz[ALARM_N_BUF];
+    alarm_sizes(h->alarm.n, h->alarm.ring, (size_t)h->alarm_batch, sz);
+    void *dst[ALARM_N_BUF];
+    alarm_buffers(h->alarm, dst);
+    const void *src[ALARM_N_BUF] = {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal};
+    for (int k = 0; k < ALARM_N_BUF; ++k)
         if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
     CU(cudaStreamSynchronize(h->stream));
     return 0;

@@ -8,7 +8,8 @@
 //   env_post_instance    the rest of BatchedEnv.step behind the solve;
 //   env_reset_instance   BatchedEnv.reset_instances (with the library's part, b200pf_series_reset_instances, and the opponent's).
 // With line alerts bound (b200pf_alert.cuh), the post body updates the alert state and the AlertReward after the step's attack,
-// and the reset body resets them.
+// and the reset body resets them; with alarms bound (b200pf_alarm.cuh), the post body registers the step's alarm once its
+// legality is known and computes the AlarmReward, and the reset body resets the attention budget.
 // The bodies are __host__ __device__: the CUDA launches run one thread per instance, a host build (tests/emu/env_emu.cpp,
 // tests/emu/opp_emu.cpp) runs the same source over the batch.  Integer arithmetic, and the opponent's fp64 operations explicitly
 // rounded: the two builds are bit-identical by construction.
@@ -17,6 +18,7 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "b200pf_alarm.cuh"
 #include "b200pf_alert.cuh"
 #include "b200pf_opp.cuh"
 
@@ -263,8 +265,8 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     }
 }
 
-// the rest of BatchedEnv.step behind the solve, for instance i (al: NULL or the line alerts)
-ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *al = nullptr) {
+// the rest of BatchedEnv.step behind the solve, for instance i (al: NULL or the line alerts, am: NULL or the alarms)
+ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr) {
     const int nl = a.n_line, ns = a.n_sub;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const bool live = a.done[i] == 0;
@@ -329,6 +331,14 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
             else al->reward_out[i] = 0.0;
         } else al->reward_out[i] = 0.0;
     }
+    const bool alarms = am && am->n;
+    if (alarms) {                                             // an instance finished before the step keeps its alarm state
+        if (live && !a.from_reset) {
+            alarm_register_instance(*am, i, a.current_step[i], a.is_illegal[i] != 0);
+            if (am->reward && newly) alarm_reward_instance(*am, i, a.current_step[i], disc);
+            else am->reward_out[i] = 0.0;
+        } else { am->illegal[i] = 0; am->reward_out[i] = 0.0; }
+    }
     if (a.obs_in) {                                           // BatchedEnv.observe_inputs
         int32_t *h = a.obs_in + (size_t)i * a.obs_stride;
         for (int l = 0; l < nl; ++l) h[l] = lc[l];
@@ -336,14 +346,16 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
         h[nl + ns] = a.current_step[i]; h[nl + ns + 1] = a.stamp;
         h[nl + ns + 2] = (a.is_illegal[i] ? 1 : 0) + (a.done[i] ? 2 : 0) + (a.obs_reset[i] ? 4 : 0);
         if (alerts) alert_obs_record(*al, i, h + nl + ns + 3);
+        if (alarms) alarm_obs_record(*am, i, a.current_step[i], h + nl + ns + 3 + (alerts ? 6 * al->n + 1 : 0));
     }
 }
 
 // BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
 ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
-                                      const OppMultiArgs *m = nullptr, const AlertArgs *al = nullptr) {
+                                      const OppMultiArgs *m = nullptr, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr) {
     if (!a.reset_mask[i]) return;
     if (al && al->n) alert_reset_instance(*al, i);
+    if (am && am->n) alarm_reset_instance(*am, i);
     if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
     if (o && g && o->kind == OPP_GEOMETRIC) opp_geo_reset_instance(*o, *g, i);
     if (o && m && o->kind == OPP_GEOMETRIC_MULTI) opp_multi_reset_instance(*m, i);
@@ -374,6 +386,7 @@ ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o 
         for (int j = 0; j < nl + a.n_sub + 1; ++j) h[j] = 0;
         h[nl + a.n_sub + 2] = 4;
         if (al && al->n) alert_obs_record(*al, i, h + nl + a.n_sub + 3);
+        if (am && am->n) alarm_obs_record(*am, i, 0, h + nl + a.n_sub + 3 + (al && al->n ? 6 * al->n + 1 : 0));
     }
 }
 
@@ -396,15 +409,16 @@ __global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o,
     env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al) {
+__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al, AlarmArgs am) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_post_instance(a, i, al.n ? &al : nullptr);
+    if (i < a.batch) env_post_instance(a, i, al.n ? &al : nullptr, am.n ? &am : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, AlertArgs al) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, AlertArgs al, AlarmArgs am) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < a.batch)
-        env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr, al.n ? &al : nullptr);
+        env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr, al.n ? &al : nullptr,
+                           am.n ? &am : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

@@ -6,7 +6,7 @@
 //                        list of the environment's observation class (CompleteObservation.attr_list_vect, completeObservation.py:140-212,
 //                        or a subset); every attribute as float32, in the order given;
 //   reward               RedispReward (grid2op/Reward/redispReward.py:141-211) or L2RPNReward (l2RPNReward.py:52-77).
-// Without redispatching, curtailment, storage actions, alarms or detachment these attributes hold the values the
+// Without redispatching, curtailment, storage actions or detachment these attributes hold the values the
 // reference produces when the features are unused.  The overflow counters timestep_overflow / timestep_protection_engaged
 // (baseEnv.py:3361-3370, counted even under NO_OVERFLOW_DISCONNECTION) are kept here, per instance, because the series kernels
 // only count while their protections are on.
@@ -78,9 +78,10 @@ struct ObsArgs {
     int reward_kind;
     double max_regret, reward_min, reward_illegal, dts_hours;
     // per-instance host inputs: int32 [batch][host_stride] = cooldown_line[n_line] | cooldown_sub[n_sub] | current_step | stamp | flags,
-    // then with line alerts (n_alert > 0) the 6 n_alert + 1 alert values of alert_obs_record (b200pf_alert.cuh)
+    // then with line alerts (n_alert > 0) the 6 n_alert + 1 alert values of alert_obs_record (b200pf_alert.cuh), then with alarms
+    // (n_alarm > 0) the n_alarm + 4 alarm values of alarm_obs_record (b200pf_alarm.cuh)
     const int32_t *host;
-    int host_stride, n_alert;
+    int host_stride, n_alert, n_alarm;
     // device state of the observation layer
     int32_t *ts_over, *ts_prot;                         // [batch][n_line]
     int32_t *stamp;                                     // [batch]: host stamp of the step the counters were last advanced for
@@ -110,6 +111,9 @@ struct ObsRec {
         sh_p = sto_v + a.n_sto; sh_q = sh_p + a.n_shunt; sh_v = sh_q + a.n_shunt;
     }
 };
+
+// first alarm value of an instance's host record
+OBS_HD inline int obs_alarm_off(const ObsArgs &a) { return a.n_line + a.n_sub + 3 + (a.n_alert ? 6 * a.n_alert + 1 : 0); }
 
 // value j of attribute source `src` for one instance (go: the game-over observation, BaseObservation.set_game_over)
 OBS_HD inline float obs_value(const ObsArgs &a, const ObsRec &R, int inst, int src, int j, bool go, int row, int sc,
@@ -151,7 +155,18 @@ OBS_HD inline float obs_value(const ObsArgs &a, const ObsRec &R, int inst, int s
     }
     case OS_GEN_P_BEFORE_CURTAIL: return (go || !a.gen_renewable[j]) ? 0.f : rec[R.unit_p + a.n_hidden + j];   // renewables only
     case OS_CURTAILMENT_LIMIT: case OS_CURTAILMENT_LIMIT_EFFECTIVE: return 1.f;
-    case OS_TIME_SINCE_LAST_ALARM: return -1.f;
+    // alarms (n_alarm > 0): the game-over observation shows no alarm (last_alarm 0, not -1), a budget of 0, and the reward's
+    // is_alarm_used; an ordinary one never sets was_alarm_used_after_game_over (BaseObservation._update_alarm, set_game_over)
+    case OS_IS_ALARM_ILLEGAL: return (go || !a.n_alarm) ? 0.f : (float)hin[obs_alarm_off(a)];
+    case OS_TIME_SINCE_LAST_ALARM: return (go || !a.n_alarm) ? -1.f : (float)hin[obs_alarm_off(a) + 1];
+    case OS_LAST_ALARM: return go ? 0.f : (float)hin[obs_alarm_off(a) + 2 + j];
+    case OS_ATTENTION_BUDGET: {
+        if (go || !a.n_alarm) return 0.f;
+        union { int32_t u; float f; } b;
+        b.u = hin[obs_alarm_off(a) + 2 + a.n_alarm];
+        return b.f;
+    }
+    case OS_WAS_ALARM_USED_AFTER_GAME_OVER: return (go && a.n_alarm) ? (float)hin[obs_alarm_off(a) + 3 + a.n_alarm] : 0.f;
     // line alerts (n_alert > 0): the game-over observation clears the alerts, their durations and the total, shows no attack,
     // and keeps attack_under_alert / was_alert_used_after_attack (BaseObservation.set_game_over, then update_after_reward)
     case OS_ACTIVE_ALERT: return go ? 0.f : (float)hin[a.n_line + a.n_sub + 3 + j];
@@ -178,7 +193,7 @@ OBS_HD inline float obs_value(const ObsArgs &a, const ObsRec &R, int inst, int s
     }
     case OS_GEN_P_DELTA: return go ? 0.f : rec[R.unit_p + a.n_hidden + j] - crow[2 * a.n_load + j];
     case OS_TS_PROTECTION_ENGAGED: return go ? 0.f : (float)tspr[j];
-    default: return 0.f;          // dispatch, storage power, curtailment, alarms, detachment: features unused
+    default: return 0.f;          // dispatch, storage power, curtailment, detachment: features unused
     }
 }
 

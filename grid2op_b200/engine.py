@@ -43,6 +43,7 @@ ABI_SYMBOLS = (
     "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
     "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state",
     "b200pf_alert_bind", "b200pf_alert_get_state", "b200pf_alert_set_state",
+    "b200pf_alarm_bind", "b200pf_alarm_get_state", "b200pf_alarm_set_state",
 )
 
 
@@ -77,7 +78,7 @@ class ObsDesc(C.Structure):
         ("gen_cost", C.c_void_p), ("gen_renewable", C.c_void_p), ("redisp_available", C.c_int32),
         ("sto_charge0", C.c_void_p), ("sto_loss_step", C.c_void_p), ("reward_kind", C.c_int32),
         ("max_regret", C.c_double), ("reward_min", C.c_double), ("reward_illegal", C.c_double), ("dts_hours", C.c_double),
-        ("soft_thr", C.c_float), ("n_alert", C.c_int32),
+        ("soft_thr", C.c_float), ("n_alert", C.c_int32), ("n_alarm", C.c_int32),
     ]
 
 
@@ -119,6 +120,15 @@ class OppMultiDesc(C.Structure):
         ("logq_hazard", C.c_double), ("logq_recovery", C.c_double), ("recovery_min", C.c_int32), ("cap", C.c_int32),
         ("episode_max_time", C.c_void_p), ("mt", C.c_void_p), ("mt_pos", C.c_void_p), ("wait", C.c_void_p), ("dur", C.c_void_p),
         ("actr", C.c_void_p), ("fails", C.c_void_p), ("attack_lines", C.c_void_p),
+    ]
+
+
+class AlarmDesc(C.Structure):
+    """``b200pf_alarm_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("n_zone", C.c_int32), ("zone_mask", C.c_void_p), ("max_budget", C.c_float), ("budget_per_ts", C.c_float),
+        ("alarm_cost", C.c_float), ("init_budget", C.c_float), ("best_time", C.c_int32), ("window_size", C.c_int32),
+        ("reward", C.c_int32), ("raise_alarm", C.c_void_p), ("reward_out", C.c_void_p), ("is_alarm_illegal", C.c_void_p),
     ]
 
 
@@ -195,6 +205,7 @@ def make_obs_desc(t: dict):
     d.max_regret, d.reward_min, d.reward_illegal, d.dts_hours = r["max_regret"], r["reward_min"], r["reward_illegal"], r["dts_hours"]
     d.soft_thr = float(t["soft_thr"])
     d.n_alert = int(t.get("n_alert", 0))
+    d.n_alarm = int(t.get("n_alarm", 0))
     return d, keep
 
 
@@ -306,11 +317,15 @@ def load_library():
     lib.b200pf_alert_bind.argtypes = [vp, C.POINTER(AlertDesc)]
     lib.b200pf_alert_get_state.argtypes = [vp] + [vp] * 12
     lib.b200pf_alert_set_state.argtypes = [vp] + [vp] * 12
+    lib.b200pf_alarm_bind.argtypes = [vp, C.POINTER(AlarmDesc)]
+    lib.b200pf_alarm_get_state.argtypes = [vp] + [vp] * 10
+    lib.b200pf_alarm_set_state.argtypes = [vp] + [vp] * 10
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
                "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
                "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state", "b200pf_alert_bind",
-               "b200pf_alert_get_state", "b200pf_alert_set_state"):
+               "b200pf_alert_get_state", "b200pf_alert_set_state", "b200pf_alarm_bind", "b200pf_alarm_get_state",
+               "b200pf_alarm_set_state"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -882,6 +897,33 @@ class PowerFlowEngine:
         from .alert import ALERT_STATE
         a = [np.ascontiguousarray(s[k], dt) for k, dt in ALERT_STATE]
         self._check(self.lib.b200pf_alert_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_alert_set_state")
+
+    def alarm_bind(self, a, d_raise: int, d_reward: int, d_illegal: int):
+        """alarms of the device environment (``b200pf_alarm_bind``): ``a`` a :class:`grid2op_b200.alarm.BatchedAlarms` (zones,
+        constants), caller-owned device buffers uint8 [B, n] (the step's raise_alarm), float64 [B] (AlarmReward) and uint8 [B]
+        (is_alarm_illegal)"""
+        zm = np.ascontiguousarray(a.zone_mask, np.uint32)
+        d = AlarmDesc(n_zone=int(a.n), zone_mask=zm.ctypes.data, max_budget=float(a.max_budget), budget_per_ts=float(a.budget_per_ts),
+                      alarm_cost=float(a.alarm_cost), init_budget=float(a.init_budget), best_time=int(a.best_time),
+                      window_size=int(a.window), reward=int(a.reward), raise_alarm=int(d_raise), reward_out=int(d_reward),
+                      is_alarm_illegal=int(d_illegal))
+        self._check(self.lib.b200pf_alarm_bind(self.h, C.byref(d)), "b200pf_alarm_bind")
+        self._alarm_shape = (int(a.n), int(a.ring))
+
+    def alarm_get_state(self):
+        """-> the alarm state of every instance, the arrays of :data:`grid2op_b200.alarm.ALARM_STATE`"""
+        from .alarm import ALARM_STATE
+        B = self._series_batch
+        n, R = getattr(self, "_alarm_shape", (0, 0))                        # (unbound: the library refuses the call)
+        shapes = dict(last=(B, n), last_ok=(B, n), ring_step=(B, R), ring_mask=(B, R))
+        s = {k: np.empty(shapes.get(k, (B,)), dt) for k, dt in ALARM_STATE}
+        self._check(self.lib.b200pf_alarm_get_state(self.h, *[_ptr(s[k]) for k, _ in ALARM_STATE]), "b200pf_alarm_get_state")
+        return s
+
+    def alarm_set_state(self, s: dict):
+        from .alarm import ALARM_STATE
+        a = [np.ascontiguousarray(s[k], dt) for k, dt in ALARM_STATE]
+        self._check(self.lib.b200pf_alarm_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_alarm_set_state")
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")

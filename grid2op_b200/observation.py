@@ -56,9 +56,9 @@ OBS_SOURCES = [
 REWARDS = {None: 0, "none": 0, "RedispReward": 1, "L2RPNReward": 2}
 
 
-def attr_sizes(gm: GridModel, n_alert: int = 0) -> Dict[str, int]:
-    """Length of every attribute in the vector of an environment without alarms (``dim_alarms = 0``) and with ``n_alert`` alertable
-    lines (``dim_alerts``; 0: an environment without alerts)."""
+def attr_sizes(gm: GridModel, n_alert: int = 0, n_alarm: int = 0) -> Dict[str, int]:
+    """Length of every attribute in the vector of an environment with ``n_alert`` alertable lines (``dim_alerts``; 0: an
+    environment without alerts) and ``n_alarm`` alarm zones (``dim_alarms``; 0: an environment without alarms)."""
     nl, ng, nld, ns, nsh, nsub = gm.n_line, gm.n_gen, gm.n_load, gm.n_storage, gm.n_shunt, gm.n_sub
     one = ("year", "month", "day", "hour_of_day", "minute_of_hour", "day_of_week", "is_alarm_illegal", "time_since_last_alarm",
            "attention_budget", "was_alarm_used_after_game_over", "current_step", "max_step", "delta_time")
@@ -78,15 +78,16 @@ def attr_sizes(gm: GridModel, n_alert: int = 0) -> Dict[str, int]:
         sz.update({k: int(n_alert) for k in ("active_alert", "attack_under_alert", "time_since_last_alert", "alert_duration",
                                               "time_since_last_attack", "was_alert_used_after_attack")})
         sz["total_number_of_alert"] = 1
+    sz["last_alarm"] = int(n_alarm)
     sz["topo_vect"] = gm.dim_topo
     sz["time_before_cooldown_sub"] = nsub
     return sz
 
 
-def obs_spec(gm: GridModel, attrs: Optional[Sequence[str]] = None, n_alert: int = 0) -> Tuple[np.ndarray, int]:
+def obs_spec(gm: GridModel, attrs: Optional[Sequence[str]] = None, n_alert: int = 0, n_alarm: int = 0) -> Tuple[np.ndarray, int]:
     """-> (int32 [n_seg, 3] rows (source, offset, length) in the order of ``attrs``, total width).  Unknown name: ValueError."""
     attrs = COMPLETE_OBSERVATION_ATTRS if attrs is None else list(attrs)
-    sz = attr_sizes(gm, n_alert)
+    sz = attr_sizes(gm, n_alert, n_alarm)
     seg, off = [], 0
     for a in attrs:
         if a not in sz:

@@ -308,7 +308,9 @@ int64_t b200pf_redo_launch_count(const b200pf_handle *h);
  * the game-over observation of BaseObservation.set_game_over, baseObservation.py:1551, and reward_min), B200PF_OBS_RESET (the
  * instance was reset: its counters restart from 0).  With line alerts (n_alert > 0, b200pf_alert_bind) the record of an instance
  * continues with 6 n_alert + 1 int32: active_alert | attack_under_alert | time_since_last_alert | alert_duration |
- * total_number_of_alert | time_since_last_attack | was_alert_used_after_attack, and the alert attributes of `seg` read them. */
+ * total_number_of_alert | time_since_last_attack | was_alert_used_after_attack, and the alert attributes of `seg` read them.
+ * With alarms (n_alarm > 0, b200pf_alarm_bind) it continues with n_alarm + 4 int32: is_alarm_illegal | time_since_last_alarm |
+ * last_alarm[n_alarm] | the attention budget's float32 bits | AlarmReward.is_alarm_used, and the five alarm attributes read them. */
 enum { B200PF_REWARD_NONE = 0, B200PF_REWARD_REDISP = 1, B200PF_REWARD_L2RPN = 2 };
 enum { B200PF_OBS_ILLEGAL = 1, B200PF_OBS_DONE = 2, B200PF_OBS_RESET = 4 };
 typedef struct b200pf_obs_desc {
@@ -326,6 +328,7 @@ typedef struct b200pf_obs_desc {
     double max_regret, reward_min, reward_illegal, dts_hours;   /* RedispReward constants; step length in hours */
     float soft_thr;                     /* SOFT_OVERFLOW_THRESHOLD (timestep_protection_engaged) */
     int32_t n_alert;                    /* dim_alerts: alert values in the host record (0: none, the record as without alerts) */
+    int32_t n_alarm;                    /* dim_alarms: alarm values in the host record (0: none, the record as without alarms) */
 } b200pf_obs_desc;
 int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *desc);
 int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float *d_reward);
@@ -507,6 +510,38 @@ int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_alert, const ui
                            const int32_t *duration, const int32_t *tsl_attack, const int32_t *under_alert, const int32_t *was_used,
                            const int32_t *total, const uint8_t *ts_attack, const uint8_t *launched, const uint8_t *current,
                            const int32_t *cur_id);
+
+/* Alarms of the device environment (grid2op's alarms of l2rpn_icaps_2021, csrc/b200pf_alarm.cuh), after b200pf_env_bind.
+ * b200pf_alarm_bind copies the zones of every line (host uint32 [n_line], bit z: zone z of the sorted zone names; every line in
+ * at least one zone) and the constants, allocates the per-instance state in the library and sets every instance to
+ * LinearAttentionBudget.reset.  From then on the post launch of b200pf_env_step, for every instance live before the step and not
+ * on a reset step, registers the step's alarm (LinearAttentionBudget.register_action, after the legality of the action) into
+ * is_alarm_illegal (uint8 [batch], caller-owned device buffer; 0 for the other instances) and, when `reward`, computes the
+ * AlarmReward into reward_out (float64 [batch], caller-owned device buffer; non-zero only on the step that ends an episode with
+ * an error, with the step's disc_lines when the protections are on).  raise_alarm: caller-owned DEVICE uint8 [batch][n_zone] the
+ * caller fills before each step (0 / 1).  b200pf_env_reset resets the attention budget of the reset instances and keeps the
+ * reward's is_alarm_used.  With the observation layer bound with the same n_alarm, the post and reset launches write the alarm
+ * values into the observe input record.  get_state / set_state copy the whole state between the device and host arrays (any
+ * pointer may be NULL): budget float32 [batch]; time_last / time_last_ok int32 [batch]; last / last_ok int32 [batch][n_zone];
+ * ring_step int32 / ring_mask uint32 [batch][best_time + window_size] (the successful alarms of the last steps, slot step %
+ * ring, step 0: empty); any_ok / used / illegal uint8 [batch] (a successful alarm this episode, is_alarm_used, the caller's
+ * is_alarm_illegal). */
+typedef struct b200pf_alarm_desc {
+    int32_t n_zone;                     /* dim_alarms, 1..32 */
+    const uint32_t *zone_mask;          /* [n_line] zones of each line */
+    float max_budget, budget_per_ts, alarm_cost, init_budget;   /* LinearAttentionBudget */
+    int32_t best_time, window_size;     /* ALARM_BEST_TIME, ALARM_WINDOW_SIZE: >= 1, their sum <= 1024 */
+    int32_t reward;                     /* compute AlarmReward (and is_alarm_used) */
+    const uint8_t *raise_alarm;         /* device [batch][n_zone] step input */
+    double *reward_out;                 /* device [batch] per-step output */
+    uint8_t *is_alarm_illegal;          /* device [batch] per-step output */
+} b200pf_alarm_desc;
+int b200pf_alarm_bind(b200pf_handle *h, const b200pf_alarm_desc *desc);
+int b200pf_alarm_get_state(b200pf_handle *h, float *budget, int32_t *time_last, int32_t *time_last_ok, int32_t *last, int32_t *last_ok,
+                           int32_t *ring_step, uint32_t *ring_mask, uint8_t *any_ok, uint8_t *used, uint8_t *illegal);
+int b200pf_alarm_set_state(b200pf_handle *h, const float *budget, const int32_t *time_last, const int32_t *time_last_ok,
+                           const int32_t *last, const int32_t *last_ok, const int32_t *ring_step, const uint32_t *ring_mask,
+                           const uint8_t *any_ok, const uint8_t *used, const uint8_t *illegal);
 
 int b200pf_sync(b200pf_handle *h);
 /* cudaStream_t of the handle as an integer (for event timing by the caller) */
