@@ -10,6 +10,7 @@
 #include "b200pf_env.cuh"
 #include "../../include/b200pf.h"
 
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -31,6 +32,12 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
         if (e__ != cudaSuccess)                                                                  \
             return fail(B200PF_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e__));     \
     } while (0)
+
+// device buffers of one layer of the device environment (observation, environment, opponent, alerts, alarms), freed together
+struct DevBufs {
+    std::vector<void *> p;
+    void release() { for (void *q : p) cudaFree(q); p.clear(); }
+};
 
 // kernel family of a launch, as b200pf_plan_stats reports it
 enum LaunchKind { KERN_NONE = 0, KERN_WARP_PIVOTING = 1, KERN_CTA_PIVOTING = 2, KERN_PLANNED_SPARSE = 3, KERN_PLANNED_BLOCK = 4 };
@@ -111,13 +118,13 @@ struct b200pf_handle {
     int last_cfg[8] = {-1, -1, -1, -1, -1, -1, -1, -1};    // template parameters of the last launch (b200pf_last_launch_config)
     // observation layer (b200pf_obs_bind / b200pf_observe)
     ObsArgs obs{}; int obs_batch = 0, obs_rows = 0;
-    std::vector<void *> obs_allocs;
+    DevBufs obs_bufs;
     int32_t *h_obs_in = nullptr, *d_obs_in = nullptr;       // pinned host record of the per-instance inputs and its device copy
     cudaEvent_t obs_ev = nullptr; bool obs_ev_pending = false;
     int64_t obs_launches = 0, obs_h2d_bytes = 0, d2h_bytes = 0;
     // device environment state (b200pf_env_bind / b200pf_env_step)
     EnvArgs env{}; int env_batch = 0;
-    std::vector<void *> env_allocs;
+    DevBufs env_bufs;
     int32_t *h_env_ctl = nullptr;                           // pinned copy of the step's control words
     std::vector<int8_t> env_mirror;                         // host mirror of the device topology the plans are looked up from
     std::vector<int32_t> env_list; std::vector<int8_t> env_rows;
@@ -126,15 +133,15 @@ struct b200pf_handle {
     int env_last_cap = 0, env_last_dirty = 0;
     // line-attack opponent of the device environment (b200pf_opp_bind)
     OppArgs opp{}; int opp_batch = 0;
-    std::vector<void *> opp_allocs;
-    OppGeoArgs opp_geo{}; bool opp_geo_bound = false;            // kind OPP_GEOMETRIC (b200pf_opp_geo_bind; its buffers in opp_allocs)
+    DevBufs opp_bufs;
+    OppGeoArgs opp_geo{}; bool opp_geo_bound = false;            // kind OPP_GEOMETRIC (b200pf_opp_geo_bind; its buffers in opp_bufs)
     OppMultiArgs opp_multi{}; bool opp_multi_bound = false;      // kind OPP_GEOMETRIC_MULTI (b200pf_opp_multi_bind; likewise)
     // line alerts of the device environment (b200pf_alert_bind)
     AlertArgs alert{}; int alert_batch = 0;
-    std::vector<void *> alert_allocs;
+    DevBufs alert_bufs;
     // alarms of the device environment (b200pf_alarm_bind)
     AlarmArgs alarm{}; int alarm_batch = 0;
-    std::vector<void *> alarm_allocs;
+    DevBufs alarm_bufs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -147,7 +154,8 @@ static int h2d_sync(b200pf_handle *h, void *dst, const void *src, size_t bytes) 
     CU(cudaStreamSynchronize(h->stream));
     return 0;
 }
-#define H2D(dst, src, bytes) do { int rc__ = h2d_sync(h, (dst), (src), (bytes)); if (rc__) return rc__; } while (0)
+#define TRY(call) do { int rc__ = (call); if (rc__) return rc__; } while (0)
+#define H2D(dst, src, bytes) TRY(h2d_sync(h, (dst), (src), (bytes)))
 
 template <typename Tp>
 static int upload(b200pf_handle *h, const Tp *src, size_t n, const Tp **dst) {
@@ -340,14 +348,14 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     for (auto &cs : h->group_stream) if (cs) { cudaStreamSynchronize(cs); cudaStreamDestroy(cs); }
     for (auto &ev : h->group_event) if (ev) cudaEventDestroy(ev);
     if (h->inst_plan_ev) cudaEventDestroy(h->inst_plan_ev);
-    for (void *p : h->obs_allocs) cudaFree(p);
+    h->obs_bufs.release();
     if (h->h_obs_in) cudaFreeHost(h->h_obs_in);
     if (h->obs_ev) cudaEventDestroy(h->obs_ev);
-    for (void *p : h->env_allocs) cudaFree(p);
+    h->env_bufs.release();
     if (h->h_env_ctl) cudaFreeHost(h->h_env_ctl);
-    for (void *p : h->opp_allocs) cudaFree(p);
-    for (void *p : h->alert_allocs) cudaFree(p);
-    for (void *p : h->alarm_allocs) cudaFree(p);
+    h->opp_bufs.release();
+    h->alert_bufs.release();
+    h->alarm_bufs.release();
     delete h;
     return 0;
 }
@@ -1687,8 +1695,83 @@ extern "C" int b200pf_plan_counters(const b200pf_handle *h, int64_t *out4) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// host code shared by the layers of the device environment (observation, environment, opponent, alerts, alarms)
+// ------------------------------------------------------------------------------------------------
+// Start of a layer's bind: drain the stream, mark the layer unbound (*batch = 0), then free its buffers.  Every bind sets its
+// *batch again last, after everything else succeeded: a bind that fails half way (an allocation, a copy, an event) leaves its
+// layer unbound, never bound over freed memory.
+static int unbind(b200pf_handle *h, int *batch, DevBufs &bufs) {
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    *batch = 0;
+    bufs.release();
+    return 0;
+}
+
+// One device buffer of a layer, owned by `bufs`: `bytes` uploaded from the host `src`, or with `src` NULL set to the byte `fill`
+// on h->stream.  `src` NULL and `fill` < 0 is an absent optional table: NULL (the kernels read it as absent), nothing allocated.
+// A zero-byte request allocates 1 byte.
+template <typename Tp>
+static int dev_alloc(b200pf_handle *h, DevBufs &bufs, Tp *&dst, size_t bytes, const void *src, int fill = -1) {
+    dst = nullptr;
+    if (!src && fill < 0) return 0;
+    void *p = nullptr;
+    CU(cudaMalloc(&p, bytes ? bytes : 1));
+    bufs.p.push_back(p);
+    dst = (Tp *)p;
+    if (src) H2D(p, src, bytes);
+    else CU(cudaMemsetAsync(p, fill, bytes ? bytes : 1, h->stream));
+    return 0;
+}
+
+// One per-instance state array of a layer: its device buffer and its bytes.  A layer's table follows the argument order of its
+// get / set entry points.
+struct StateBuf { void *dev; size_t bytes; };
+
+// b200pf_*_get_state: drain the stream, then a blocking copy of every array the caller asked for (non-NULL destination)
+template <size_t N>
+static int state_get(b200pf_handle *h, const std::array<StateBuf, N> &t, void *const (&dst)[N]) {
+    CU(cudaSetDevice(h->device));
+    CU(cudaStreamSynchronize(h->stream));
+    for (size_t k = 0; k < N; ++k)
+        if (dst[k]) { CU(cudaMemcpy(dst[k], t[k].dev, t[k].bytes, cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)t[k].bytes; }
+    return 0;
+}
+
+// b200pf_*_set_state, once the caller has validated every array it was given (so that a rejected call changes nothing): every
+// non-NULL source through h2d_sync, then one stream sync
+template <size_t N>
+static int state_set(b200pf_handle *h, const std::array<StateBuf, N> &t, const void *const (&src)[N]) {
+    CU(cudaSetDevice(h->device));
+    for (size_t k = 0; k < N; ++k)
+        if (src[k]) { H2D(t[k].dev, src[k], t[k].bytes); h->env_h2d += (int64_t)t[k].bytes; }
+    CU(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // observation layer: grid2op observation vectors + rewards of the bound series, assembled on the device (b200pf_obs.cuh)
 // ------------------------------------------------------------------------------------------------
+// the observation layer is bound to the current series (b200pf_obs_bind)
+static bool obs_bound(const b200pf_handle *h) { return h->obs_batch && h->obs_batch == h->series_batch && h->obs_rows == h->n_rows; }
+
+// ints per instance of the observe input record: the observation layer's, or the record without alerts and alarms when it is unbound
+static int obs_stride(const b200pf_handle *h) { return obs_bound(h) ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3; }
+
+// the observe launch: the bound tables over the series' current results and the input record, writing d_obs / d_reward
+static ObsArgs obs_args(const b200pf_handle *h, float *d_obs, float *d_reward) {
+    const DevGrid &g = h->g;
+    ObsArgs a = h->obs;
+    a.batch = h->obs_batch;
+    a.n_line = g.n_line; a.n_sub = g.n_sub; a.n_gen = g.n_gen; a.n_hidden = g.n_hidden; a.n_load = g.n_load; a.n_sto = g.n_sto;
+    a.n_shunt = g.n_shunt; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_out = g.n_out;
+    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
+    a.out = h->x_out ? h->x_out : h->d_out; a.rho = h->x_rho ? h->x_rho : h->d_rho; a.topo = h->d_series_topo;
+    a.t = h->d_t; a.scen = h->d_scen; a.chron = h->d_chron; a.n_rows = h->n_rows; a.th_lim = h->d_thlim;
+    a.host = h->d_obs_in; a.obs = d_obs; a.reward = d_reward;
+    return a;
+}
+
 extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
     if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
@@ -1703,79 +1786,53 @@ extern "C" int b200pf_obs_bind(b200pf_handle *h, const b200pf_obs_desc *d) {
     for (int s = 0; s < d->n_seg; ++s)
         if (d->seg[3 * s] < 0 || d->seg[3 * s] >= OS_N_SOURCES || d->seg[3 * s + 1] < 0 || d->seg[3 * s + 2] < 0 ||
             d->seg[3 * s + 1] + d->seg[3 * s + 2] > d->n_obs) return fail(B200PF_E_ARG, "observation segment out of range");
-    CU(cudaSetDevice(h->device));
-    CU(cudaStreamSynchronize(h->stream));
-    for (void *p : h->obs_allocs) cudaFree(p);
-    h->obs_allocs.clear();
+    TRY(unbind(h, &h->obs_batch, h->obs_bufs));
     if (h->h_obs_in) { cudaFreeHost(h->h_obs_in); h->h_obs_in = nullptr; }
     if (!h->obs_ev) CU(cudaEventCreateWithFlags(&h->obs_ev, cudaEventDisableTiming));
     h->obs_ev_pending = false;
-    const size_t B = (size_t)h->series_batch, R = (size_t)h->n_scen * h->n_rows, nl = (size_t)g.n_line;
-    auto dup = [&](const void *src, size_t bytes, void **dst) -> int {
-        *dst = nullptr;
-        if (!src) return 0;
-        CU(cudaMalloc(dst, bytes ? bytes : 1));
-        h->obs_allocs.push_back(*dst);
-        if (bytes) H2D(*dst, src, bytes);
-        return 0;
-    };
-    auto zeros = [&](size_t bytes, int byte, void **dst) -> int {
-        CU(cudaMalloc(dst, bytes ? bytes : 1));
-        h->obs_allocs.push_back(*dst);
-        CU(cudaMemsetAsync(*dst, byte, bytes ? bytes : 1, h->stream));
-        return 0;
-    };
+    const size_t B = (size_t)h->series_batch, R = (size_t)h->n_scen * h->n_rows, nl = (size_t)g.n_line, ng = (size_t)g.n_gen;
+    DevBufs &o = h->obs_bufs;
     ObsArgs a{};
-    void *p[17] = {};
-    int rc;
-    if ((rc = dup(d->seg, (size_t)d->n_seg * 12, &p[0])) || (rc = dup(d->calendar, R * 24, &p[1])) || (rc = dup(d->max_step, (size_t)h->n_scen * 4, &p[2])) ||
-        (rc = dup(d->maint_time, R * nl * 4, &p[3])) || (rc = dup(d->maint_dur, R * nl * 4, &p[4])) ||
-        (rc = dup(d->gen_pmin, (size_t)g.n_gen * 4, &p[5])) || (rc = dup(d->gen_pmax, (size_t)g.n_gen * 4, &p[6])) ||
-        (rc = dup(d->gen_ramp_up, (size_t)g.n_gen * 4, &p[7])) || (rc = dup(d->gen_ramp_down, (size_t)g.n_gen * 4, &p[8])) ||
-        (rc = dup(d->gen_cost, (size_t)g.n_gen * 4, &p[9])) || (rc = dup(d->gen_renewable, (size_t)g.n_gen, &p[10])) ||
-        (rc = dup(d->sto_charge0, (size_t)g.n_sto * 4, &p[11])) || (rc = dup(d->sto_loss_step, (size_t)g.n_sto * 4, &p[12])) ||
-        (rc = zeros(B * nl * 4, 0, &p[13])) || (rc = zeros(B * nl * 4, 0, &p[14])) || (rc = zeros(B * 4, 0xff, &p[15])) || (rc = zeros(B * 4, 0xff, &p[16])))
-        return rc;
-    a.seg = (const int32_t *)p[0]; a.calendar = (const int32_t *)p[1]; a.max_step = (const int32_t *)p[2];
-    a.maint_time = (const int32_t *)p[3]; a.maint_dur = (const int32_t *)p[4];
-    a.gen_pmin = (const float *)p[5]; a.gen_pmax = (const float *)p[6]; a.gen_ramp_up = (const float *)p[7]; a.gen_ramp_down = (const float *)p[8];
-    a.gen_cost = (const float *)p[9]; a.gen_renewable = (const int8_t *)p[10];
-    a.sto_charge0 = (const float *)p[11]; a.sto_loss_step = (const float *)p[12];
-    a.ts_over = (int32_t *)p[13]; a.ts_prot = (int32_t *)p[14]; a.stamp = (int32_t *)p[15]; a.go_row = (int32_t *)p[16];
+    TRY(dev_alloc(h, o, a.seg, (size_t)d->n_seg * 12, d->seg));
+    TRY(dev_alloc(h, o, a.calendar, R * 24, d->calendar));
+    TRY(dev_alloc(h, o, a.max_step, (size_t)h->n_scen * 4, d->max_step));
+    TRY(dev_alloc(h, o, a.maint_time, R * nl * 4, d->maint_time));
+    TRY(dev_alloc(h, o, a.maint_dur, R * nl * 4, d->maint_dur));
+    TRY(dev_alloc(h, o, a.gen_pmin, ng * 4, d->gen_pmin));
+    TRY(dev_alloc(h, o, a.gen_pmax, ng * 4, d->gen_pmax));
+    TRY(dev_alloc(h, o, a.gen_ramp_up, ng * 4, d->gen_ramp_up));
+    TRY(dev_alloc(h, o, a.gen_ramp_down, ng * 4, d->gen_ramp_down));
+    TRY(dev_alloc(h, o, a.gen_cost, ng * 4, d->gen_cost));
+    TRY(dev_alloc(h, o, a.gen_renewable, ng, d->gen_renewable));
+    TRY(dev_alloc(h, o, a.sto_charge0, (size_t)g.n_sto * 4, d->sto_charge0));
+    TRY(dev_alloc(h, o, a.sto_loss_step, (size_t)g.n_sto * 4, d->sto_loss_step));
+    TRY(dev_alloc(h, o, a.ts_over, B * nl * 4, nullptr, 0));
+    TRY(dev_alloc(h, o, a.ts_prot, B * nl * 4, nullptr, 0));
+    TRY(dev_alloc(h, o, a.stamp, B * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, o, a.go_row, B * 4, nullptr, 0xff));
     a.n_seg = d->n_seg; a.n_obs = d->n_obs; a.delta_time = d->delta_time; a.redisp_available = d->redisp_available;
     a.reward_kind = d->reward_kind; a.max_regret = d->max_regret; a.reward_min = d->reward_min; a.reward_illegal = d->reward_illegal;
     a.dts_hours = d->dts_hours; a.soft_thr = d->soft_thr;
     a.n_alert = d->n_alert; a.n_alarm = d->n_alarm;
     a.host_stride = g.n_line + g.n_sub + 3 + (d->n_alert ? 6 * d->n_alert + 1 : 0) + (d->n_alarm ? d->n_alarm + 4 : 0);
     if (cudaMallocHost(&h->h_obs_in, B * a.host_stride * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
-    void *din = nullptr;
-    if ((rc = zeros(B * a.host_stride * 4, 0, &din))) return rc;
-    h->d_obs_in = (int32_t *)din;
+    TRY(dev_alloc(h, o, h->d_obs_in, B * a.host_stride * 4, nullptr, 0));
     CU(cudaStreamSynchronize(h->stream));
-    h->obs = a; h->obs_batch = h->series_batch; h->obs_rows = h->n_rows;
+    h->obs = a; h->obs_rows = h->n_rows; h->obs_batch = h->series_batch;
     return 0;
 }
 
 extern "C" int b200pf_observe(b200pf_handle *h, const int32_t *host_in, float *d_obs, float *d_reward) {
     if (!h || !host_in || !d_obs) return fail(B200PF_E_ARG, "null pointer");
-    if (!h->obs_batch || h->obs_batch != h->series_batch || h->obs_rows != h->n_rows)
-        return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
+    if (!obs_bound(h)) return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
     CU(cudaSetDevice(h->device));
-    const DevGrid &g = h->g;
-    ObsArgs a = h->obs;
-    const size_t in_bytes = (size_t)h->obs_batch * a.host_stride * 4;
+    const ObsArgs a = obs_args(h, d_obs, d_reward);
+    const size_t in_bytes = (size_t)a.batch * a.host_stride * 4;
     if (h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));        // the previous copy out of the pinned record has left
     memcpy(h->h_obs_in, host_in, in_bytes);
     CU(cudaMemcpyAsync(h->d_obs_in, h->h_obs_in, in_bytes, cudaMemcpyHostToDevice, h->stream));
     CU(cudaEventRecord(h->obs_ev, h->stream));
     h->obs_ev_pending = true;
-    a.batch = h->obs_batch;
-    a.n_line = g.n_line; a.n_sub = g.n_sub; a.n_gen = g.n_gen; a.n_hidden = g.n_hidden; a.n_load = g.n_load; a.n_sto = g.n_sto;
-    a.n_shunt = g.n_shunt; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_out = g.n_out;
-    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
-    a.out = h->x_out ? h->x_out : h->d_out; a.rho = h->x_rho ? h->x_rho : h->d_rho; a.topo = h->d_series_topo;
-    a.t = h->d_t; a.scen = h->d_scen; a.chron = h->d_chron; a.n_rows = h->n_rows; a.th_lim = h->d_thlim;
-    a.host = h->d_obs_in; a.obs = d_obs; a.reward = d_reward;
     pf_kernel_observe<<<(a.batch + 3) / 4, 128, 0, h->stream>>>(a);
     CU(cudaGetLastError());
     h->obs_launches++; h->obs_h2d_bytes += (int64_t)in_bytes;
@@ -1818,6 +1875,9 @@ extern "C" int b200pf_last_launch_config(const b200pf_handle *h, int *cfg8) {
 // ------------------------------------------------------------------------------------------------
 static bool env_bound(const b200pf_handle *h) { return h->env_batch && h->env_batch == h->series_batch && h->env.topo == h->d_series_topo; }
 
+// a layer bound for `batch` instances (the opponent, the alerts, the alarms) belongs to the current environment
+static bool layer_bound(const b200pf_handle *h, int batch) { return env_bound(h) && batch == h->env_batch; }
+
 extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
     if (!h->series_batch) return fail(B200PF_E_STATE, "series not bound");
@@ -1837,26 +1897,8 @@ extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
     for (int k = 0; k < d->n_iso_seg; ++k) if (d->iso_seg[k] < 0 || d->iso_seg[k] > d->n_iso_cols) return fail(B200PF_E_ARG, "iso_seg out of range");
     const int B = h->series_batch;
     for (int i = 0; i < B; ++i) if (d->t0[i] < 0 || d->t0[i] >= h->n_rows) return fail(B200PF_E_ARG, "t0 out of range");
-    CU(cudaSetDevice(h->device));
-    CU(cudaStreamSynchronize(h->stream));
-    for (void *p : h->env_allocs) cudaFree(p);
-    h->env_allocs.clear();
-    h->env_batch = 0;
+    TRY(unbind(h, &h->env_batch, h->env_bufs));
     if (!h->h_env_ctl && cudaMallocHost(&h->h_env_ctl, ENV_CTL_WORDS * 4) != cudaSuccess) return fail(B200PF_E_CUDA, "pinned host allocation failed");
-    auto dup = [&](const void *src, size_t bytes, void **dst) -> int {
-        *dst = nullptr;
-        if (!src) return 0;
-        CU(cudaMalloc(dst, bytes ? bytes : 1));
-        h->env_allocs.push_back(*dst);
-        if (bytes) H2D(*dst, src, bytes);
-        return 0;
-    };
-    auto zeros = [&](size_t bytes, int byte, void **dst) -> int {
-        CU(cudaMalloc(dst, bytes ? bytes : 1));
-        h->env_allocs.push_back(*dst);
-        CU(cudaMemsetAsync(*dst, byte, bytes ? bytes : 1, h->stream));
-        return 0;
-    };
     std::vector<int32_t> epos, esub;           // every element of the record and its substation (b200pf_grid_max_active_buses)
     const HostGrid &hg = h->hg;
     for (int k = 0; k < hg.n_line; ++k) { epos.push_back(hg.line_or_pos[k]); esub.push_back(hg.line_or_sub[k]); }
@@ -1865,87 +1907,85 @@ extern "C" int b200pf_env_bind(b200pf_handle *h, const b200pf_env_desc *d) {
     for (int k = 0; k < hg.n_load; ++k) { epos.push_back(hg.load_pos[k]); esub.push_back(hg.load_sub[k]); }
     for (int k = 0; k < hg.n_sto; ++k) { epos.push_back(hg.sto_pos[k]); esub.push_back(hg.sto_sub[k]); }
     for (int k = 0; k < hg.n_shunt; ++k) { epos.push_back(hg.dim_topo + k); esub.push_back(hg.sh_sub[k]); }
-    const size_t R = (size_t)h->n_scen * h->n_rows * g.n_line, nl = (size_t)g.n_line, nt = (size_t)g.n_topo_in;
+    const size_t R = (size_t)h->n_scen * h->n_rows * g.n_line, nl = (size_t)g.n_line, nt = (size_t)g.n_topo_in, Bs = (size_t)B;
+    DevBufs &o = h->env_bufs;
     EnvArgs a{};
-    void *p[32] = {};
-    int rc;
-    if ((rc = dup(d->sub_pos, (size_t)g.n_sub * d->max_sub * 4, &p[0])) || (rc = dup(d->line_of_pos, (size_t)g.dim_topo * 4, &p[1])) ||
-        (rc = dup(d->other_end_pos, (size_t)g.dim_topo * 4, &p[2])) || (rc = dup(epos.data(), epos.size() * 4, &p[3])) ||
-        (rc = dup(esub.data(), esub.size() * 4, &p[4])) || (rc = dup(d->maint, R, &p[5])) || (rc = dup(d->haz, R, &p[6])) ||
-        (rc = dup(d->maint_time, R * 4, &p[7])) || (rc = dup(d->maint_dur, R * 4, &p[8])) || (rc = dup(d->haz_dur, R * 4, &p[9])) ||
-        (rc = dup(d->iso_cols, (size_t)d->n_iso_cols * 4, &p[10])) || (rc = dup(d->iso_seg, (size_t)d->n_iso_seg * 4, &p[11])) ||
-        (rc = dup(d->topo0, (size_t)B * nt, &p[12])) || (rc = dup(d->t0, (size_t)B * 4, &p[13])) ||
-        (rc = zeros((size_t)B * nl, 0, &p[14])) || (rc = zeros((size_t)B * 4, 0xff, &p[15])) || (rc = zeros((size_t)B * 4, 0, &p[16])) ||
-        (rc = zeros((size_t)B, 0, &p[17])) || (rc = zeros((size_t)B, 1, &p[18])) || (rc = zeros((size_t)B, 1, &p[19])) ||
-        (rc = zeros((size_t)B * 4, 0, &p[20])) || (rc = zeros((size_t)B * 4, 0, &p[21])) || (rc = zeros((size_t)B * nt, 0, &p[22])) ||
-        (rc = zeros(ENV_CTL_WORDS * 4, 0, &p[23])))
-        return rc;
+    TRY(dev_alloc(h, o, a.sub_pos, (size_t)g.n_sub * d->max_sub * 4, d->sub_pos));
+    TRY(dev_alloc(h, o, a.line_of_pos, (size_t)g.dim_topo * 4, d->line_of_pos));
+    TRY(dev_alloc(h, o, a.other_end_pos, (size_t)g.dim_topo * 4, d->other_end_pos));
+    TRY(dev_alloc(h, o, a.elem_pos, epos.size() * 4, epos.data()));
+    TRY(dev_alloc(h, o, a.elem_sub, esub.size() * 4, esub.data()));
+    TRY(dev_alloc(h, o, a.maint, R, d->maint));
+    TRY(dev_alloc(h, o, a.haz, R, d->haz));
+    TRY(dev_alloc(h, o, a.maint_time, R * 4, d->maint_time));
+    TRY(dev_alloc(h, o, a.maint_dur, R * 4, d->maint_dur));
+    TRY(dev_alloc(h, o, a.haz_dur, R * 4, d->haz_dur));
+    TRY(dev_alloc(h, o, a.iso_cols, (size_t)d->n_iso_cols * 4, d->iso_cols));
+    TRY(dev_alloc(h, o, a.iso_seg, (size_t)d->n_iso_seg * 4, d->iso_seg));
+    TRY(dev_alloc(h, o, a.topo0, Bs * nt, d->topo0));
+    TRY(dev_alloc(h, o, a.t0, Bs * 4, d->t0));
+    TRY(dev_alloc(h, o, a.aff_l, Bs * nl, nullptr, 0));
+    TRY(dev_alloc(h, o, a.aff_s, Bs * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, o, a.row_used, Bs * 4, nullptr, 0));
+    TRY(dev_alloc(h, o, a.stale, Bs, nullptr, 0));
+    TRY(dev_alloc(h, o, a.cap_dirty, Bs, nullptr, 1));
+    TRY(dev_alloc(h, o, a.obs_reset, Bs, nullptr, 1));
+    TRY(dev_alloc(h, o, a.nb_inst, Bs * 4, nullptr, 0));
+    TRY(dev_alloc(h, o, a.copy_list, Bs * 4, nullptr, 0));
+    TRY(dev_alloc(h, o, a.copy_rows, Bs * nt, nullptr, 0));
+    TRY(dev_alloc(h, o, a.ctl, ENV_CTL_WORDS * 4, nullptr, 0));
     a.batch = B;
     a.n_line = g.n_line; a.n_sub = g.n_sub; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_busbar = g.n_busbar; a.n_slot = g.n_slot;
     a.max_sub = d->max_sub; a.n_rows = h->n_rows;
-    a.sub_pos = (const int32_t *)p[0]; a.line_of_pos = (const int32_t *)p[1]; a.other_end_pos = (const int32_t *)p[2];
-    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
-    a.elem_pos = (const int32_t *)p[3]; a.elem_sub = (const int32_t *)p[4]; a.n_elem = (int)epos.size();
+    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos; a.n_elem = (int)epos.size();
     a.cd_line = d->cd_line; a.cd_sub = d->cd_sub; a.cd_reco = d->cd_reco;
-    a.maint = (const uint8_t *)p[5]; a.haz = (const uint8_t *)p[6];
-    a.maint_time = (const int32_t *)p[7]; a.maint_dur = (const int32_t *)p[8]; a.haz_dur = (const int32_t *)p[9];
-    a.iso_cols = (const int32_t *)p[10]; a.iso_seg = (const int32_t *)p[11]; a.n_iso_seg = d->n_iso_seg; a.n_iso_cols = d->n_iso_cols;
-    a.topo0 = (const int8_t *)p[12]; a.t0 = (const int32_t *)p[13]; a.scen = h->d_scen;
+    a.n_iso_seg = d->n_iso_seg; a.n_iso_cols = d->n_iso_cols; a.scen = h->d_scen;
     a.topo = h->d_series_topo; a.t = h->d_t;
     a.lib_done = h->d_done; a.pcount = h->d_pcount; a.ts_over = h->d_tsover; a.lib_disc = h->d_disc; a.trip = h->d_trip; a.incdone = h->d_incdone;
     a.last_bus = d->last_bus; a.line_cd = d->line_cd; a.sub_cd = d->sub_cd; a.done = d->done; a.is_illegal = d->is_illegal;
     a.newly_done = d->newly_done; a.current_step = d->current_step; a.status_out = d->status;
-    a.aff_l = (uint8_t *)p[14]; a.aff_s = (int32_t *)p[15]; a.row_used = (int32_t *)p[16];
-    a.stale = (uint8_t *)p[17]; a.cap_dirty = (uint8_t *)p[18]; a.obs_reset = (uint8_t *)p[19];
-    a.nb_inst = (int32_t *)p[20]; a.copy_list = (int32_t *)p[21]; a.copy_rows = (int8_t *)p[22]; a.ctl = (int32_t *)p[23];
     // the stale flags start set: the first step that refreshes the plans copies every row into the mirror
-    CU(cudaMemsetAsync(a.stale, 1, (size_t)B, h->stream));
+    CU(cudaMemsetAsync(a.stale, 1, Bs, h->stream));
     CU(cudaStreamSynchronize(h->stream));
-    h->env = a; h->env_batch = B;
-    h->env_mirror.assign((size_t)B * nt, 0);
-    h->env_topo0.assign(d->topo0, d->topo0 + (size_t)B * nt);
+    h->env = a;
+    h->env_mirror.assign(Bs * nt, 0);
+    h->env_topo0.assign(d->topo0, d->topo0 + Bs * nt);
+    h->env_batch = B;
     return 0;
 }
 
 static inline unsigned env_grid(int n) { return (unsigned)((n + 127) / 128); }
 
-// the opponent the env launches run: the bound one, or none (kind OPP_NONE)
-static OppArgs env_opp(const b200pf_handle *h);
-
-// the line alerts the env launches run (n = 0: none), reading the attacked lines the opponent of the same launches writes
-static AlertArgs env_alert(const b200pf_handle *h) {
-    if (!h->alert_batch || h->alert_batch != h->env_batch) return AlertArgs{};
-    AlertArgs al = h->alert;
-    const OppArgs o = env_opp(h);
-    if (o.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound) { al.attack = h->opp_multi.attack_lines; al.attack_stride = h->opp_multi.n_area; }
-    else if (o.kind != OPP_NONE) { al.attack = o.attack_line; al.attack_stride = 1; }
-    return al;
-}
-
-// the alarms the env launches run (n = 0: none)
-static AlarmArgs env_alarm(const b200pf_handle *h) {
-    if (!h->alarm_batch || h->alarm_batch != h->env_batch) return AlarmArgs{};
-    return h->alarm;
-}
-
-// the observe input record the env launches write: NULL when the observation layer is not bound to this series; an error
-// when its alert or alarm values do not match the bound alerts or alarms
-static int env_obs_record(const b200pf_handle *h, const AlertArgs &al, const AlarmArgs &am, int32_t **rec, int *stride) {
-    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
-    *rec = obs ? h->d_obs_in : nullptr;
-    *stride = obs ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3;
-    if (obs && h->obs.n_alert != al.n)
+// What the env launches run besides the EnvArgs: the bound opponent (kind OPP_NONE: none), the line alerts (n = 0: none; they read
+// the attacked lines the opponent of the same launches writes), the alarms (n = 0: none) and the observe input record (NULL when
+// the observation layer is not bound to this series).  An error when a GeometricOpponent lacks its schedules, a multi-area one its
+// areas, or when the observation layer's alert or alarm values do not match the bound alerts or alarms.
+struct EnvLayers { OppArgs opp; AlertArgs al; AlarmArgs am; int32_t *obs_rec; int obs_stride; };
+static int env_layers(const b200pf_handle *h, EnvLayers *l) {
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
+    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
+        return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
+    l->opp = OppArgs{};
+    if (layer_bound(h, h->opp_batch)) {
+        l->opp = h->opp;
+        l->opp.rho = h->x_rho ? h->x_rho : h->d_rho;                  // what the previous step wrote
+    }
+    l->al = AlertArgs{};
+    if (layer_bound(h, h->alert_batch)) {
+        l->al = h->alert;
+        if (l->opp.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound) { l->al.attack = h->opp_multi.attack_lines; l->al.attack_stride = h->opp_multi.n_area; }
+        else if (l->opp.kind != OPP_NONE) { l->al.attack = l->opp.attack_line; l->al.attack_stride = 1; }
+    }
+    l->am = layer_bound(h, h->alarm_batch) ? h->alarm : AlarmArgs{};
+    const bool obs = obs_bound(h);
+    l->obs_rec = obs ? h->d_obs_in : nullptr;
+    l->obs_stride = obs_stride(h);
+    if (obs && h->obs.n_alert != l->al.n)
         return fail(B200PF_E_STATE, "the observation layer and the line alerts disagree on dim_alerts (b200pf_obs_bind / b200pf_alert_bind)");
-    if (obs && h->obs.n_alarm != am.n)
+    if (obs && h->obs.n_alarm != l->am.n)
         return fail(B200PF_E_STATE, "the observation layer and the alarms disagree on dim_alarms (b200pf_obs_bind / b200pf_alarm_bind)");
     return 0;
-}
-
-static OppArgs env_opp(const b200pf_handle *h) {
-    if (!h->opp_batch || h->opp_batch != h->env_batch) return OppArgs{};
-    OppArgs o = h->opp;
-    o.rho = h->x_rho ? h->x_rho : h->d_rho;                  // what the previous step wrote
-    return o;
 }
 
 extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
@@ -1954,15 +1994,9 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
-    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
-        return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
-    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
-        return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
-    const AlertArgs al = env_alert(h);
-    const AlarmArgs am = env_alarm(h);
-    int32_t *obs_rec; int obs_stride;
-    if (int rc0 = env_obs_record(h, al, am, &obs_rec, &obs_stride)) return rc0;
+    EnvLayers l;
+    TRY(env_layers(h, &l));
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -1978,7 +2012,7 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
         pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi);
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi);
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2023,8 +2057,8 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     // 6. trips, isolated busbars, cooldowns, game over, the observe layer's input record
     a.status = h->x_status ? h->x_status : h->d_status;
     a.disc = h->prot ? h->d_disc : nullptr;
-    a.obs_in = obs_rec; a.obs_stride = obs_stride; a.stamp = stamp;
-    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, al, am);
+    a.obs_in = l.obs_rec; a.obs_stride = l.obs_stride; a.stamp = stamp;
+    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, l.al, l.am);
     CU(cudaGetLastError());
     h->env_steps++;
     return 0;
@@ -2033,22 +2067,16 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
 extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const int32_t *d_rows) {
     if (!h || !d_mask) return fail(B200PF_E_ARG, "null pointer");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
-    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
-        return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
-    if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC_MULTI && !h->opp_multi_bound)
-        return fail(B200PF_E_STATE, "GeometricOpponentMultiArea bound without its areas (b200pf_opp_multi_bind)");
-    const AlertArgs al = env_alert(h);
-    const AlarmArgs am = env_alarm(h);
-    int32_t *obs_rec; int obs_stride;
-    if (int rc0 = env_obs_record(h, al, am, &obs_rec, &obs_stride)) return rc0;
+    EnvLayers l;
+    TRY(env_layers(h, &l));
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
     const size_t nt = (size_t)g.n_topo_in;
     EnvArgs a = h->env;
     a.reset_mask = d_mask; a.reset_rows = d_rows;
-    a.obs_in = obs_rec; a.obs_stride = obs_stride;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, env_opp(h), h->opp_geo, h->opp_multi, al, am);
+    a.obs_in = l.obs_rec; a.obs_stride = l.obs_stride;
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.al, l.am);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel
@@ -2075,16 +2103,10 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
 extern "C" int b200pf_env_get_state(b200pf_handle *h, int8_t *topo, int32_t *t, int32_t *nb_inst, uint8_t *cap_dirty, uint8_t *obs_reset) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
-    CU(cudaSetDevice(h->device));
     const size_t B = (size_t)h->env_batch, nt = (size_t)h->g.n_topo_in;
-    CU(cudaStreamSynchronize(h->stream));
-    if (topo) CU(cudaMemcpy(topo, h->d_series_topo, B * nt, cudaMemcpyDeviceToHost));
-    if (t) CU(cudaMemcpy(t, h->d_t, B * 4, cudaMemcpyDeviceToHost));
-    if (nb_inst) CU(cudaMemcpy(nb_inst, h->env.nb_inst, B * 4, cudaMemcpyDeviceToHost));
-    if (cap_dirty) CU(cudaMemcpy(cap_dirty, h->env.cap_dirty, B, cudaMemcpyDeviceToHost));
-    if (obs_reset) CU(cudaMemcpy(obs_reset, h->env.obs_reset, B, cudaMemcpyDeviceToHost));
-    h->env_d2h += (int64_t)((topo ? B * nt : 0) + (t ? B * 4 : 0) + (nb_inst ? B * 4 : 0) + (cap_dirty ? B : 0) + (obs_reset ? B : 0));
-    return 0;
+    const std::array<StateBuf, 5> tab = {{{h->d_series_topo, B * nt}, {h->d_t, B * 4}, {h->env.nb_inst, B * 4}, {h->env.cap_dirty, B},
+                                          {h->env.obs_reset, B}}};
+    return state_get(h, tab, {topo, t, nb_inst, cap_dirty, obs_reset});
 }
 
 extern "C" int b200pf_env_set_state(b200pf_handle *h, const int8_t *topo, const int32_t *nb_inst, const uint8_t *cap_dirty, const uint8_t *obs_reset,
@@ -2093,22 +2115,15 @@ extern "C" int b200pf_env_set_state(b200pf_handle *h, const int8_t *topo, const 
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     CU(cudaSetDevice(h->device));
     const size_t B = (size_t)h->env_batch, nt = (size_t)h->g.n_topo_in;
-    if (topo) {
-        H2D(h->d_series_topo, topo, B * nt);
-        h->env_mirror.assign(topo, topo + B * nt);
-        CU(cudaMemsetAsync(h->env.stale, 0, B, h->stream));
-    }
-    if (nb_inst) H2D(h->env.nb_inst, nb_inst, B * 4);
-    if (cap_dirty) H2D(h->env.cap_dirty, cap_dirty, B);
-    if (obs_reset) H2D(h->env.obs_reset, obs_reset, B);
-    const bool obs = h->obs_batch == h->series_batch && h->obs_rows == h->n_rows && h->d_obs_in;
-    const size_t rec = B * (size_t)(obs ? h->obs.host_stride : h->g.n_line + h->g.n_sub + 3) * 4;
-    if (obs_in && obs) {
-        if (h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));        // (b200pf_observe's copy into the same record has left)
-        H2D(h->d_obs_in, obs_in, rec);
-    }
-    CU(cudaStreamSynchronize(h->stream));
-    h->env_h2d += (int64_t)((topo ? B * nt : 0) + (nb_inst ? B * 4 : 0) + (cap_dirty ? B : 0) + (obs_reset ? B : 0) + (obs_in && obs ? rec : 0));
+    const bool obs = obs_bound(h);
+    // a new topology leaves no row stale: the flags are cleared on the stream ahead of the copies (state_set's closing sync
+    // covers it), the host mirror is patched once the topology is on the device
+    if (topo) CU(cudaMemsetAsync(h->env.stale, 0, B, h->stream));
+    if (obs_in && obs && h->obs_ev_pending) CU(cudaEventSynchronize(h->obs_ev));    // (b200pf_observe's copy into the same record has left)
+    const std::array<StateBuf, 5> tab = {{{h->d_series_topo, B * nt}, {h->env.nb_inst, B * 4}, {h->env.cap_dirty, B}, {h->env.obs_reset, B},
+                                          {h->d_obs_in, B * (size_t)obs_stride(h) * 4}}};
+    TRY(state_set(h, tab, {topo, nb_inst, cap_dirty, obs_reset, obs ? obs_in : nullptr}));
+    if (topo) h->env_mirror.assign(topo, topo + B * nt);
     return 0;
 }
 
@@ -2123,19 +2138,10 @@ extern "C" int b200pf_env_pointers(b200pf_handle *h, int8_t **d_topo, int32_t **
 
 extern "C" int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_reward) {
     if (!h || !d_obs) return fail(B200PF_E_ARG, "null pointer");
-    if (!h->obs_batch || h->obs_batch != h->series_batch || h->obs_rows != h->n_rows)
-        return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
+    if (!obs_bound(h)) return fail(B200PF_E_STATE, "observation not bound to the current series (b200pf_obs_bind)");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     CU(cudaSetDevice(h->device));
-    const DevGrid &g = h->g;
-    ObsArgs a = h->obs;
-    a.batch = h->obs_batch;
-    a.n_line = g.n_line; a.n_sub = g.n_sub; a.n_gen = g.n_gen; a.n_hidden = g.n_hidden; a.n_load = g.n_load; a.n_sto = g.n_sto;
-    a.n_shunt = g.n_shunt; a.dim_topo = g.dim_topo; a.n_topo_in = g.n_topo_in; a.n_out = g.n_out;
-    a.line_or_pos = g.line_or_pos; a.line_ex_pos = g.line_ex_pos;
-    a.out = h->x_out ? h->x_out : h->d_out; a.rho = h->x_rho ? h->x_rho : h->d_rho; a.topo = h->d_series_topo;
-    a.t = h->d_t; a.scen = h->d_scen; a.chron = h->d_chron; a.n_rows = h->n_rows; a.th_lim = h->d_thlim;
-    a.host = h->d_obs_in; a.obs = d_obs; a.reward = d_reward;
+    const ObsArgs a = obs_args(h, d_obs, d_reward);
     pf_kernel_observe<<<(a.batch + 3) / 4, 128, 0, h->stream>>>(a);
     CU(cudaGetLastError());
     EnvArgs e = h->env;                  // the reset flags have been consumed
@@ -2143,6 +2149,24 @@ extern "C" int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_re
     pf_kernel_env_observed<<<env_grid(e.batch), 128, 0, h->stream>>>(e);
     CU(cudaGetLastError());
     h->obs_launches++;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// line-attack opponent of the device environment (b200pf_opp.cuh)
+// ------------------------------------------------------------------------------------------------
+// the checks of the opponent's random states and schedule counters, shared by its binds and its set_state entry points: n MT19937
+// positions; n blocks of schedule counters, `stride` ints each (OPP_GEO_CTR, or OPP_AREA_CTR per area: the same leading counters)
+static int mt_pos_check(const int32_t *mt_pos, size_t n) {
+    for (size_t k = 0; mt_pos && k < n; ++k)
+        if (mt_pos[k] < 0 || mt_pos[k] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
+    return 0;
+}
+static int sched_ctr_check(const int32_t *ctr, size_t n, int stride, int cap) {
+    for (size_t k = 0; ctr && k < n; ++k) {
+        const int32_t *c = ctr + k * stride;
+        if (c[OPP_GEO_N] < 0 || c[OPP_GEO_N] > cap || c[OPP_GEO_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
+    }
     return 0;
 }
 
@@ -2158,33 +2182,15 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
         return fail(B200PF_E_ARG, "bad opponent description");
     for (int k = 0; k < d->n_attack; ++k) if (d->lines[k] < 0 || d->lines[k] >= g.n_line) return fail(B200PF_E_ARG, "attacked line out of range");
     const int B = h->env_batch;
-    for (int i = 0; i < B; ++i) if (d->mt_pos[i] < 0 || d->mt_pos[i] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
-    CU(cudaSetDevice(h->device));
-    CU(cudaStreamSynchronize(h->stream));
-    for (void *p : h->opp_allocs) cudaFree(p);
-    h->opp_allocs.clear();
-    h->opp_batch = 0;
+    TRY(mt_pos_check(d->mt_pos, (size_t)B));
+    TRY(unbind(h, &h->opp_batch, h->opp_bufs));
     h->opp_geo = OppGeoArgs{}; h->opp_geo_bound = false;
     h->opp_multi = OppMultiArgs{}; h->opp_multi_bound = false;
-    auto dev = [&](const void *src, size_t bytes, void **dst) -> int {
-        CU(cudaMalloc(dst, bytes));
-        h->opp_allocs.push_back(*dst);
-        if (src) H2D(*dst, src, bytes);
-        return 0;
-    };
-    void *p[6] = {};
-    int rc;
-    if ((rc = dev(d->lines, (size_t)d->n_attack * 4, &p[0])) ||
-        (rc = dev(d->rho_norm, (size_t)d->n_attack * 8, &p[1])) || (rc = dev(nullptr, (size_t)B, &p[2])) ||
-        (rc = dev(nullptr, (size_t)B * OPP_CTR * 4, &p[3])) || (rc = dev(d->mt, (size_t)B * OPP_MT_N * 4, &p[4])) ||
-        (rc = dev(d->mt_pos, (size_t)B * 4, &p[5])))
-        return rc;
     OppArgs o{};
-    o.kind = d->kind; o.n_attack = d->n_attack; o.lines = (const int32_t *)p[0]; o.rho_norm = (const double *)p[1];
+    o.kind = d->kind; o.n_attack = d->n_attack;
     o.attack_period = d->attack_period; o.attack_duration = d->attack_duration; o.attack_cooldown = d->attack_cooldown;
     o.budget_per_ts = d->budget_per_ts; o.init_budget = d->init_budget;
-    o.budget = d->budget; o.budget64 = (uint8_t *)p[2]; o.ctr = (int32_t *)p[3]; o.mt = (uint32_t *)p[4]; o.mt_pos = (int32_t *)p[5];
-    o.attack_line = d->attack_line; o.attack_dur = d->attack_dur;
+    o.budget = d->budget; o.attack_line = d->attack_line; o.attack_dur = d->attack_dur;
     // every instance starts from OpponentSpace.reset()
     std::vector<double> bud((size_t)B, (double)d->init_budget);
     std::vector<int32_t> ctr((size_t)B * OPP_CTR);
@@ -2192,135 +2198,90 @@ extern "C" int b200pf_opp_bind(b200pf_handle *h, const b200pf_opp_desc *d) {
         ctr[(size_t)i * OPP_CTR + OPP_CTR_DURATION] = 0; ctr[(size_t)i * OPP_CTR + OPP_CTR_COOLDOWN] = d->attack_cooldown;
         ctr[(size_t)i * OPP_CTR + OPP_CTR_LAST] = -1; ctr[(size_t)i * OPP_CTR + OPP_CTR_NEXT] = OPP_NEXT_UNSET;
     }
+    DevBufs &ob = h->opp_bufs;
+    TRY(dev_alloc(h, ob, o.lines, (size_t)d->n_attack * 4, d->lines));
+    TRY(dev_alloc(h, ob, o.rho_norm, (size_t)d->n_attack * 8, d->rho_norm, 0));    // (read by kind OPP_WEIGHTED_RANDOM only)
+    TRY(dev_alloc(h, ob, o.budget64, (size_t)B, nullptr, 0));
+    TRY(dev_alloc(h, ob, o.ctr, ctr.size() * 4, ctr.data()));
+    TRY(dev_alloc(h, ob, o.mt, (size_t)B * OPP_MT_N * 4, d->mt));
+    TRY(dev_alloc(h, ob, o.mt_pos, (size_t)B * 4, d->mt_pos));
     H2D(o.budget, bud.data(), (size_t)B * 8);
-    H2D(o.ctr, ctr.data(), ctr.size() * 4);
-    CU(cudaMemsetAsync(o.budget64, 0, (size_t)B, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     h->opp = o; h->opp_batch = B;
     return 0;
 }
 
-static bool opp_bound(const b200pf_handle *h) { return env_bound(h) && h->opp_batch == h->env_batch; }
+// the opponent's per-instance state, in the argument order of b200pf_opp_get_state / _set_state
+static std::array<StateBuf, 5> opp_state(const b200pf_handle *h) {
+    const OppArgs &o = h->opp;
+    const size_t B = (size_t)h->opp_batch;
+    return {{{o.budget, B * 8}, {o.budget64, B}, {o.ctr, B * OPP_CTR * 4}, {o.mt, B * OPP_MT_N * 4}, {o.mt_pos, B * 4}}};
+}
 
 extern "C" int b200pf_opp_get_state(b200pf_handle *h, double *budget, uint8_t *budget64, int32_t *ctr, uint32_t *mt, int32_t *mt_pos) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!opp_bound(h)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
-    CU(cudaSetDevice(h->device));
-    const size_t B = (size_t)h->opp_batch;
-    const OppArgs &o = h->opp;
-    CU(cudaStreamSynchronize(h->stream));
-    if (budget) CU(cudaMemcpy(budget, o.budget, B * 8, cudaMemcpyDeviceToHost));
-    if (budget64) CU(cudaMemcpy(budget64, o.budget64, B, cudaMemcpyDeviceToHost));
-    if (ctr) CU(cudaMemcpy(ctr, o.ctr, B * OPP_CTR * 4, cudaMemcpyDeviceToHost));
-    if (mt) CU(cudaMemcpy(mt, o.mt, B * OPP_MT_N * 4, cudaMemcpyDeviceToHost));
-    if (mt_pos) CU(cudaMemcpy(mt_pos, o.mt_pos, B * 4, cudaMemcpyDeviceToHost));
-    h->env_d2h += (int64_t)((budget ? B * 8 : 0) + (budget64 ? B : 0) + (ctr ? B * OPP_CTR * 4 : 0) + (mt ? B * OPP_MT_N * 4 : 0) + (mt_pos ? B * 4 : 0));
-    return 0;
+    if (!layer_bound(h, h->opp_batch)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
+    return state_get(h, opp_state(h), {budget, budget64, ctr, mt, mt_pos});
 }
 
 extern "C" int b200pf_opp_set_state(b200pf_handle *h, const double *budget, const uint8_t *budget64, const int32_t *ctr, const uint32_t *mt,
                                     const int32_t *mt_pos) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!opp_bound(h)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
-    const size_t B = (size_t)h->opp_batch;
-    if (mt_pos) for (size_t i = 0; i < B; ++i) if (mt_pos[i] < 0 || mt_pos[i] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
-    CU(cudaSetDevice(h->device));
-    const OppArgs &o = h->opp;
-    if (budget) H2D(o.budget, budget, B * 8);
-    if (budget64) H2D(o.budget64, budget64, B);
-    if (ctr) H2D(o.ctr, ctr, B * OPP_CTR * 4);
-    if (mt) H2D(o.mt, mt, B * OPP_MT_N * 4);
-    if (mt_pos) H2D(o.mt_pos, mt_pos, B * 4);
-    CU(cudaStreamSynchronize(h->stream));
-    h->env_h2d += (int64_t)((budget ? B * 8 : 0) + (budget64 ? B : 0) + (ctr ? B * OPP_CTR * 4 : 0) + (mt ? B * OPP_MT_N * 4 : 0) + (mt_pos ? B * 4 : 0));
-    return 0;
+    if (!layer_bound(h, h->opp_batch)) return fail(B200PF_E_STATE, "no opponent bound to the current environment (b200pf_opp_bind)");
+    TRY(mt_pos_check(mt_pos, (size_t)h->opp_batch));
+    return state_set(h, opp_state(h), {budget, budget64, ctr, mt, mt_pos});
 }
 
 extern "C" int b200pf_opp_geo_bind(b200pf_handle *h, const b200pf_opp_geo_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
-    if (!opp_bound(h) || h->opp.kind != OPP_GEOMETRIC) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_bind, kind 3)");
+    if (!layer_bound(h, h->opp_batch) || h->opp.kind != OPP_GEOMETRIC) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_bind, kind 3)");
     if (!d->weights || !d->episode_max_time || !d->wait || !d->dur || !d->gctr || d->cap < 1 || d->recovery_min < 0 ||
         !(d->p_hazard > 0.0 && d->p_hazard <= 1.0) || !(d->p_recovery > 0.0 && d->p_recovery <= 1.0))
         return fail(B200PF_E_ARG, "bad GeometricOpponent description");
     const int B = h->opp_batch;
-    for (int i = 0; i < B; ++i) {
-        const int32_t *gc = d->gctr + (size_t)i * OPP_GEO_CTR;
-        if (gc[OPP_GEO_N] < 0 || gc[OPP_GEO_N] > d->cap || gc[OPP_GEO_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
-    }
+    TRY(sched_ctr_check(d->gctr, (size_t)B, OPP_GEO_CTR, d->cap));
     CU(cudaSetDevice(h->device));
     CU(cudaStreamSynchronize(h->stream));
     const size_t n_sched = (size_t)B * (size_t)d->cap * 4;
-    void *p[5] = {};
-    const void *src[5] = {d->weights, d->episode_max_time, d->wait, d->dur, d->gctr};
-    const size_t bytes[5] = {(size_t)h->opp.n_attack * 8, (size_t)B * 4, n_sched, n_sched, (size_t)B * OPP_GEO_CTR * 4};
-    for (int k = 0; k < 5; ++k) {
-        CU(cudaMalloc(&p[k], bytes[k]));
-        h->opp_allocs.push_back(p[k]);
-        H2D(p[k], src[k], bytes[k]);
-    }
-    CU(cudaStreamSynchronize(h->stream));
+    DevBufs &ob = h->opp_bufs;
     OppGeoArgs g{};
-    g.weights = (const double *)p[0]; g.p_hazard = d->p_hazard; g.p_recovery = d->p_recovery;
+    TRY(dev_alloc(h, ob, g.weights, (size_t)h->opp.n_attack * 8, d->weights));
+    TRY(dev_alloc(h, ob, g.emt, (size_t)B * 4, d->episode_max_time));
+    TRY(dev_alloc(h, ob, g.wait, n_sched, d->wait));
+    TRY(dev_alloc(h, ob, g.dur, n_sched, d->dur));
+    TRY(dev_alloc(h, ob, g.gctr, (size_t)B * OPP_GEO_CTR * 4, d->gctr));
+    CU(cudaStreamSynchronize(h->stream));
+    g.p_hazard = d->p_hazard; g.p_recovery = d->p_recovery;
     g.logq_hazard = d->logq_hazard; g.logq_recovery = d->logq_recovery; g.recovery_min = d->recovery_min; g.cap = d->cap;
-    g.emt = (const int32_t *)p[1]; g.wait = (int32_t *)p[2]; g.dur = (int32_t *)p[3]; g.gctr = (int32_t *)p[4];
     h->opp_geo = g; h->opp_geo_bound = true;
     return 0;
 }
 
-static bool opp_geo_ready(const b200pf_handle *h) { return opp_bound(h) && h->opp.kind == OPP_GEOMETRIC && h->opp_geo_bound; }
+static bool opp_geo_ready(const b200pf_handle *h) { return layer_bound(h, h->opp_batch) && h->opp.kind == OPP_GEOMETRIC && h->opp_geo_bound; }
+
+// the GeometricOpponent's per-instance state, in the argument order of b200pf_opp_geo_get_state / _set_state
+static std::array<StateBuf, 3> opp_geo_state(const b200pf_handle *h) {
+    const OppGeoArgs &g = h->opp_geo;
+    const size_t B = (size_t)h->opp_batch, n_sched = B * (size_t)g.cap * 4;
+    return {{{g.wait, n_sched}, {g.dur, n_sched}, {g.gctr, B * OPP_GEO_CTR * 4}}};
+}
 
 extern "C" int b200pf_opp_geo_get_state(b200pf_handle *h, int32_t *wait, int32_t *dur, int32_t *gctr) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!opp_geo_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_geo_bind)");
-    CU(cudaSetDevice(h->device));
-    const OppGeoArgs &g = h->opp_geo;
-    const size_t B = (size_t)h->opp_batch, n_sched = B * (size_t)g.cap * 4;
-    CU(cudaStreamSynchronize(h->stream));
-    if (wait) CU(cudaMemcpy(wait, g.wait, n_sched, cudaMemcpyDeviceToHost));
-    if (dur) CU(cudaMemcpy(dur, g.dur, n_sched, cudaMemcpyDeviceToHost));
-    if (gctr) CU(cudaMemcpy(gctr, g.gctr, B * OPP_GEO_CTR * 4, cudaMemcpyDeviceToHost));
-    h->env_d2h += (int64_t)((wait ? n_sched : 0) + (dur ? n_sched : 0) + (gctr ? B * OPP_GEO_CTR * 4 : 0));
-    return 0;
+    return state_get(h, opp_geo_state(h), {wait, dur, gctr});
 }
 
 extern "C" int b200pf_opp_geo_set_state(b200pf_handle *h, const int32_t *wait, const int32_t *dur, const int32_t *gctr) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!opp_geo_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponent bound (b200pf_opp_geo_bind)");
-    const OppGeoArgs &g = h->opp_geo;
-    const size_t B = (size_t)h->opp_batch, n_sched = B * (size_t)g.cap * 4;
-    if (gctr)
-        for (size_t i = 0; i < B; ++i) {
-            const int32_t *gc = gctr + i * OPP_GEO_CTR;
-            if (gc[OPP_GEO_N] < 0 || gc[OPP_GEO_N] > g.cap || gc[OPP_GEO_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
-        }
-    CU(cudaSetDevice(h->device));
-    if (wait) H2D(g.wait, wait, n_sched);
-    if (dur) H2D(g.dur, dur, n_sched);
-    if (gctr) H2D(g.gctr, gctr, B * OPP_GEO_CTR * 4);
-    CU(cudaStreamSynchronize(h->stream));
-    h->env_h2d += (int64_t)((wait ? n_sched : 0) + (dur ? n_sched : 0) + (gctr ? B * OPP_GEO_CTR * 4 : 0));
-    return 0;
-}
-
-// the per-area arrays of a GeometricOpponentMultiArea: MT words, MT positions, waiting times, durations, counters, previous_fails
-static void opp_multi_sizes(const OppMultiArgs &m, size_t B, size_t out[6]) {
-    const size_t ba = B * (size_t)m.n_area;
-    out[0] = ba * OPP_MT_N * 4; out[1] = ba * 4; out[2] = out[3] = ba * (size_t)m.cap * 4; out[4] = ba * OPP_AREA_CTR * 4; out[5] = B * 4;
-}
-
-static int opp_multi_check(const int32_t *mt_pos, const int32_t *actr, int cap, size_t ba) {
-    for (size_t k = 0; mt_pos && k < ba; ++k)
-        if (mt_pos[k] < 0 || mt_pos[k] > OPP_MT_N) return fail(B200PF_E_ARG, "random state position out of range");
-    for (size_t k = 0; actr && k < ba; ++k) {
-        const int32_t *ac = actr + k * OPP_AREA_CTR;
-        if (ac[OPP_AREA_N] < 0 || ac[OPP_AREA_N] > cap || ac[OPP_AREA_COUNTER] < 0) return fail(B200PF_E_ARG, "schedule counters out of range");
-    }
-    return 0;
+    TRY(sched_ctr_check(gctr, (size_t)h->opp_batch, OPP_GEO_CTR, h->opp_geo.cap));
+    return state_set(h, opp_geo_state(h), {wait, dur, gctr});
 }
 
 extern "C" int b200pf_opp_multi_bind(b200pf_handle *h, const b200pf_opp_multi_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
-    if (!opp_bound(h) || h->opp.kind != OPP_GEOMETRIC_MULTI)
+    if (!layer_bound(h, h->opp_batch) || h->opp.kind != OPP_GEOMETRIC_MULTI)
         return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_bind, kind 4)");
     if (d->n_area < 1 || d->n_area > OPP_MAX_AREA || !d->area_off || !d->weights || !d->episode_max_time || !d->mt || !d->mt_pos ||
         !d->wait || !d->dur || !d->actr || !d->fails || !d->attack_lines || d->cap < 1 || d->recovery_min < 0 ||
@@ -2330,81 +2291,60 @@ extern "C" int b200pf_opp_multi_bind(b200pf_handle *h, const b200pf_opp_multi_de
     for (int k = 0; k < d->n_area; ++k)
         if (d->area_off[k + 1] <= d->area_off[k]) return fail(B200PF_E_ARG, "empty area");
     const int B = h->opp_batch;
-    int rc = opp_multi_check(d->mt_pos, d->actr, d->cap, (size_t)B * d->n_area);
-    if (rc) return rc;
+    const size_t ba = (size_t)B * d->n_area, n_sched = ba * (size_t)d->cap * 4;
+    TRY(mt_pos_check(d->mt_pos, ba));
+    TRY(sched_ctr_check(d->actr, ba, OPP_AREA_CTR, d->cap));
     OppMultiArgs m{};
     m.n_area = d->n_area;
     for (int k = 0; k <= d->n_area; ++k) m.area_off[k] = d->area_off[k];
     m.p_hazard = d->p_hazard; m.p_recovery = d->p_recovery; m.logq_hazard = d->logq_hazard; m.logq_recovery = d->logq_recovery;
     m.recovery_min = d->recovery_min; m.cap = d->cap; m.attack_lines = d->attack_lines;
-    size_t sz[6];
-    opp_multi_sizes(m, (size_t)B, sz);
     CU(cudaSetDevice(h->device));
     CU(cudaStreamSynchronize(h->stream));
-    void *p[8] = {};
-    const void *src[8] = {d->weights, d->episode_max_time, d->mt, d->mt_pos, d->wait, d->dur, d->actr, d->fails};
-    const size_t bytes[8] = {(size_t)h->opp.n_attack * 8, (size_t)B * 4, sz[0], sz[1], sz[2], sz[3], sz[4], sz[5]};
-    for (int k = 0; k < 8; ++k) {
-        CU(cudaMalloc(&p[k], bytes[k]));
-        h->opp_allocs.push_back(p[k]);
-        H2D(p[k], src[k], bytes[k]);
-    }
+    DevBufs &ob = h->opp_bufs;
+    TRY(dev_alloc(h, ob, m.weights, (size_t)h->opp.n_attack * 8, d->weights));
+    TRY(dev_alloc(h, ob, m.emt, (size_t)B * 4, d->episode_max_time));
+    TRY(dev_alloc(h, ob, m.mt, ba * OPP_MT_N * 4, d->mt));
+    TRY(dev_alloc(h, ob, m.mt_pos, ba * 4, d->mt_pos));
+    TRY(dev_alloc(h, ob, m.wait, n_sched, d->wait));
+    TRY(dev_alloc(h, ob, m.dur, n_sched, d->dur));
+    TRY(dev_alloc(h, ob, m.actr, ba * OPP_AREA_CTR * 4, d->actr));
+    TRY(dev_alloc(h, ob, m.fails, (size_t)B * 4, d->fails));
     CU(cudaStreamSynchronize(h->stream));
-    m.weights = (const double *)p[0]; m.emt = (const int32_t *)p[1]; m.mt = (uint32_t *)p[2]; m.mt_pos = (int32_t *)p[3];
-    m.wait = (int32_t *)p[4]; m.dur = (int32_t *)p[5]; m.actr = (int32_t *)p[6]; m.fails = (int32_t *)p[7];
     h->opp_multi = m; h->opp_multi_bound = true;
     return 0;
 }
 
-static bool opp_multi_ready(const b200pf_handle *h) { return opp_bound(h) && h->opp.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound; }
+static bool opp_multi_ready(const b200pf_handle *h) { return layer_bound(h, h->opp_batch) && h->opp.kind == OPP_GEOMETRIC_MULTI && h->opp_multi_bound; }
+
+// the GeometricOpponentMultiArea's per-instance state, in the argument order of b200pf_opp_multi_get_state / _set_state: MT
+// words, MT positions, waiting times, durations, counters of every area, previous_fails
+static std::array<StateBuf, 6> opp_multi_state(const b200pf_handle *h) {
+    const OppMultiArgs &m = h->opp_multi;
+    const size_t B = (size_t)h->opp_batch, ba = B * (size_t)m.n_area, n_sched = ba * (size_t)m.cap * 4;
+    return {{{m.mt, ba * OPP_MT_N * 4}, {m.mt_pos, ba * 4}, {m.wait, n_sched}, {m.dur, n_sched}, {m.actr, ba * OPP_AREA_CTR * 4}, {m.fails, B * 4}}};
+}
 
 extern "C" int b200pf_opp_multi_get_state(b200pf_handle *h, uint32_t *mt, int32_t *mt_pos, int32_t *wait, int32_t *dur, int32_t *actr,
                                           int32_t *fails) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!opp_multi_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_multi_bind)");
-    CU(cudaSetDevice(h->device));
-    const OppMultiArgs &m = h->opp_multi;
-    size_t sz[6];
-    opp_multi_sizes(m, (size_t)h->opp_batch, sz);
-    void *dst[6] = {mt, mt_pos, wait, dur, actr, fails};
-    const void *src[6] = {m.mt, m.mt_pos, m.wait, m.dur, m.actr, m.fails};
-    CU(cudaStreamSynchronize(h->stream));
-    for (int k = 0; k < 6; ++k)
-        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
-    return 0;
+    return state_get(h, opp_multi_state(h), {mt, mt_pos, wait, dur, actr, fails});
 }
 
 extern "C" int b200pf_opp_multi_set_state(b200pf_handle *h, const uint32_t *mt, const int32_t *mt_pos, const int32_t *wait, const int32_t *dur,
                                           const int32_t *actr, const int32_t *fails) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!opp_multi_ready(h)) return fail(B200PF_E_STATE, "no GeometricOpponentMultiArea bound (b200pf_opp_multi_bind)");
-    const OppMultiArgs &m = h->opp_multi;
-    int rc = opp_multi_check(mt_pos, actr, m.cap, (size_t)h->opp_batch * m.n_area);
-    if (rc) return rc;
-    size_t sz[6];
-    opp_multi_sizes(m, (size_t)h->opp_batch, sz);
-    void *dst[6] = {m.mt, m.mt_pos, m.wait, m.dur, m.actr, m.fails};
-    const void *src[6] = {mt, mt_pos, wait, dur, actr, fails};
-    CU(cudaSetDevice(h->device));
-    for (int k = 0; k < 6; ++k)
-        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
-    CU(cudaStreamSynchronize(h->stream));
-    return 0;
+    const size_t ba = (size_t)h->opp_batch * h->opp_multi.n_area;
+    TRY(mt_pos_check(mt_pos, ba));
+    TRY(sched_ctr_check(actr, ba, OPP_AREA_CTR, h->opp_multi.cap));
+    return state_set(h, opp_multi_state(h), {mt, mt_pos, wait, dur, actr, fails});
 }
 
-// the alert state buffers in the order of b200pf_alert_get_state / _set_state, and their bytes for a batch of B
-enum { ALERT_N_BUF = 12 };
-static void alert_buffers(const AlertArgs &al, void *p[ALERT_N_BUF]) {
-    void *q[ALERT_N_BUF] = {al.last_alert, al.already, al.tsl_alert, al.duration, al.tsl_attack, al.under_alert, al.was_used, al.total,
-                            al.ts_attack, al.launched, al.current, al.cur_id};
-    for (int k = 0; k < ALERT_N_BUF; ++k) p[k] = q[k];
-}
-static void alert_sizes(int n, int ring, size_t B, size_t out[ALERT_N_BUF]) {
-    const size_t bn = B * (size_t)n;
-    const size_t s[ALERT_N_BUF] = {bn, bn, bn * 4, bn * 4, bn * 4, bn * 4, bn * 4, B * 4, bn * ring, bn * ring, bn, B * 4};
-    for (int k = 0; k < ALERT_N_BUF; ++k) out[k] = s[k];
-}
-
+// ------------------------------------------------------------------------------------------------
+// line alerts and alarms of the device environment (b200pf_alert.cuh, b200pf_alarm.cuh)
+// ------------------------------------------------------------------------------------------------
 extern "C" int b200pf_alert_bind(b200pf_handle *h, const b200pf_alert_desc *d) {
     if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
@@ -2414,11 +2354,7 @@ extern "C" int b200pf_alert_bind(b200pf_handle *h, const b200pf_alert_desc *d) {
         if (d->lines[k] < 0 || d->lines[k] >= h->g.n_line) return fail(B200PF_E_ARG, "alertable line out of range");
         for (int j = 0; j < k; ++j) if (d->lines[j] == d->lines[k]) return fail(B200PF_E_ARG, "alertable line listed twice");
     }
-    CU(cudaSetDevice(h->device));
-    CU(cudaStreamSynchronize(h->stream));
-    for (void *p : h->alert_allocs) cudaFree(p);
-    h->alert_allocs.clear();
-    h->alert_batch = 0;
+    TRY(unbind(h, &h->alert_batch, h->alert_bufs));
     const size_t B = (size_t)h->env_batch;
     AlertArgs al{};
     al.n = d->n_alert; al.window = d->window; al.ring = d->window + 2; al.reward = d->reward ? 1 : 0;
@@ -2427,47 +2363,44 @@ extern "C" int b200pf_alert_bind(b200pf_handle *h, const b200pf_alert_desc *d) {
     al.max_no_blackout = (double)d->reward_max_no_blackout;
     al.diff_no_blackout = (double)(d->reward_min_no_blackout - d->reward_max_no_blackout);    // float32, as AlertReward
     al.raise = d->raise_alert; al.reward_out = d->reward_out;
-    void *lines = nullptr;
-    CU(cudaMalloc(&lines, (size_t)al.n * 4));
-    h->alert_allocs.push_back(lines);
-    H2D(lines, d->lines, (size_t)al.n * 4);
-    al.lines = (const int32_t *)lines;
-    size_t sz[ALERT_N_BUF];
-    alert_sizes(al.n, al.ring, B, sz);
-    void *p[ALERT_N_BUF];
-    for (int k = 0; k < ALERT_N_BUF; ++k) {
-        CU(cudaMalloc(&p[k], sz[k]));
-        h->alert_allocs.push_back(p[k]);
-    }
-    al.last_alert = (uint8_t *)p[0]; al.already = (uint8_t *)p[1]; al.tsl_alert = (int32_t *)p[2]; al.duration = (int32_t *)p[3];
-    al.tsl_attack = (int32_t *)p[4]; al.under_alert = (int32_t *)p[5]; al.was_used = (int32_t *)p[6]; al.total = (int32_t *)p[7];
-    al.ts_attack = (uint8_t *)p[8]; al.launched = (uint8_t *)p[9]; al.current = (uint8_t *)p[10]; al.cur_id = (int32_t *)p[11];
+    const size_t bn = B * (size_t)al.n, br = bn * (size_t)al.ring;
+    DevBufs &ob = h->alert_bufs;
+    TRY(dev_alloc(h, ob, al.lines, (size_t)al.n * 4, d->lines));
     // every instance starts from _reset_alert + AlertReward.reset: zeros, and -1 for the two "time since" counters
-    for (int k = 0; k < ALERT_N_BUF; ++k) CU(cudaMemsetAsync(p[k], (k == 2 || k == 4) ? 0xff : 0, sz[k], h->stream));
+    TRY(dev_alloc(h, ob, al.last_alert, bn, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.already, bn, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.tsl_alert, bn * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, al.duration, bn * 4, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.tsl_attack, bn * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, al.under_alert, bn * 4, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.was_used, bn * 4, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.total, B * 4, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.ts_attack, br, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.launched, br, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.current, bn, nullptr, 0));
+    TRY(dev_alloc(h, ob, al.cur_id, B * 4, nullptr, 0));
     CU(cudaMemsetAsync(al.reward_out, 0, B * 8, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     h->alert = al; h->alert_batch = (int)B;
     return 0;
 }
 
-static bool alert_bound(const b200pf_handle *h) { return env_bound(h) && h->alert_batch == h->env_batch; }
+// the alerts' per-instance state, in the argument order of b200pf_alert_get_state / _set_state
+static std::array<StateBuf, 12> alert_state(const b200pf_handle *h) {
+    const AlertArgs &al = h->alert;
+    const size_t B = (size_t)h->alert_batch, bn = B * (size_t)al.n, br = bn * (size_t)al.ring;
+    return {{{al.last_alert, bn}, {al.already, bn}, {al.tsl_alert, bn * 4}, {al.duration, bn * 4}, {al.tsl_attack, bn * 4},
+             {al.under_alert, bn * 4}, {al.was_used, bn * 4}, {al.total, B * 4}, {al.ts_attack, br}, {al.launched, br}, {al.current, bn},
+             {al.cur_id, B * 4}}};
+}
 
 extern "C" int b200pf_alert_get_state(b200pf_handle *h, uint8_t *last_alert, uint8_t *already, int32_t *tsl_alert, int32_t *duration,
                                       int32_t *tsl_attack, int32_t *under_alert, int32_t *was_used, int32_t *total, uint8_t *ts_attack,
                                       uint8_t *launched, uint8_t *current, int32_t *cur_id) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!alert_bound(h)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
-    CU(cudaSetDevice(h->device));
-    size_t sz[ALERT_N_BUF];
-    alert_sizes(h->alert.n, h->alert.ring, (size_t)h->alert_batch, sz);
-    void *src[ALERT_N_BUF];
-    alert_buffers(h->alert, src);
-    void *dst[ALERT_N_BUF] = {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack, launched,
-                              current, cur_id};
-    CU(cudaStreamSynchronize(h->stream));
-    for (int k = 0; k < ALERT_N_BUF; ++k)
-        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
-    return 0;
+    if (!layer_bound(h, h->alert_batch)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
+    return state_get(h, alert_state(h), {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack,
+                                         launched, current, cur_id});
 }
 
 extern "C" int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_alert, const uint8_t *already, const int32_t *tsl_alert,
@@ -2475,34 +2408,11 @@ extern "C" int b200pf_alert_set_state(b200pf_handle *h, const uint8_t *last_aler
                                       const int32_t *total, const uint8_t *ts_attack, const uint8_t *launched, const uint8_t *current,
                                       const int32_t *cur_id) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!alert_bound(h)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
+    if (!layer_bound(h, h->alert_batch)) return fail(B200PF_E_STATE, "no line alerts bound to the current environment (b200pf_alert_bind)");
     const size_t B = (size_t)h->alert_batch;
     if (cur_id) for (size_t i = 0; i < B; ++i) if (cur_id[i] < 0 || cur_id[i] >= h->alert.ring) return fail(B200PF_E_ARG, "ring index out of range");
-    CU(cudaSetDevice(h->device));
-    size_t sz[ALERT_N_BUF];
-    alert_sizes(h->alert.n, h->alert.ring, B, sz);
-    void *dst[ALERT_N_BUF];
-    alert_buffers(h->alert, dst);
-    const void *src[ALERT_N_BUF] = {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack, launched,
-                                    current, cur_id};
-    for (int k = 0; k < ALERT_N_BUF; ++k)
-        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
-    CU(cudaStreamSynchronize(h->stream));
-    return 0;
-}
-
-// the alarm state buffers in the order of b200pf_alarm_get_state / _set_state (the last one, is_alarm_illegal, is the caller's),
-// and their bytes for a batch of B
-enum { ALARM_N_BUF = 10 };
-static void alarm_buffers(const AlarmArgs &am, void *p[ALARM_N_BUF]) {
-    void *q[ALARM_N_BUF] = {am.budget, am.time_last, am.time_last_ok, am.last, am.last_ok, am.ring_step, am.ring_mask, am.any_ok,
-                            am.used, am.illegal};
-    for (int k = 0; k < ALARM_N_BUF; ++k) p[k] = q[k];
-}
-static void alarm_sizes(int n, int ring, size_t B, size_t out[ALARM_N_BUF]) {
-    const size_t bn = B * (size_t)n * 4, br = B * (size_t)ring * 4;
-    const size_t s[ALARM_N_BUF] = {B * 4, B * 4, B * 4, bn, bn, br, br, B, B, B};
-    for (int k = 0; k < ALARM_N_BUF; ++k) out[k] = s[k];
+    return state_set(h, alert_state(h), {last_alert, already, tsl_alert, duration, tsl_attack, under_alert, was_used, total, ts_attack,
+                                         launched, current, cur_id});
 }
 
 extern "C" int b200pf_alarm_bind(b200pf_handle *h, const b200pf_alarm_desc *d) {
@@ -2514,36 +2424,27 @@ extern "C" int b200pf_alarm_bind(b200pf_handle *h, const b200pf_alarm_desc *d) {
     const uint32_t zones = d->n_zone == 32 ? 0xffffffffu : (1u << d->n_zone) - 1u;
     for (int l = 0; l < h->g.n_line; ++l)
         if (!d->zone_mask[l] || (d->zone_mask[l] & ~zones)) return fail(B200PF_E_ARG, "a line in no zone, or in a zone past n_zone");
-    CU(cudaSetDevice(h->device));
-    CU(cudaStreamSynchronize(h->stream));
-    for (void *p : h->alarm_allocs) cudaFree(p);
-    h->alarm_allocs.clear();
-    h->alarm_batch = 0;
+    TRY(unbind(h, &h->alarm_batch, h->alarm_bufs));
     const size_t B = (size_t)h->env_batch;
     AlarmArgs am{};
     am.n = d->n_zone; am.n_line = h->g.n_line;
     am.max_budget = d->max_budget; am.budget_per_ts = d->budget_per_ts; am.alarm_cost = d->alarm_cost; am.init_budget = d->init_budget;
     am.best_time = d->best_time; am.window = d->window_size; am.ring = d->best_time + d->window_size; am.reward = d->reward ? 1 : 0;
     am.raise = d->raise_alarm; am.reward_out = d->reward_out; am.illegal = d->is_alarm_illegal;
-    void *zm = nullptr;
-    CU(cudaMalloc(&zm, (size_t)am.n_line * 4));
-    h->alarm_allocs.push_back(zm);
-    H2D(zm, d->zone_mask, (size_t)am.n_line * 4);
-    am.zone_mask = (const uint32_t *)zm;
-    size_t sz[ALARM_N_BUF];
-    alarm_sizes(am.n, am.ring, B, sz);
-    void *p[ALARM_N_BUF];
-    for (int k = 0; k < ALARM_N_BUF - 1; ++k) {
-        CU(cudaMalloc(&p[k], sz[k]));
-        h->alarm_allocs.push_back(p[k]);
-    }
-    am.budget = (float *)p[0]; am.time_last = (int32_t *)p[1]; am.time_last_ok = (int32_t *)p[2]; am.last = (int32_t *)p[3];
-    am.last_ok = (int32_t *)p[4]; am.ring_step = (int32_t *)p[5]; am.ring_mask = (uint32_t *)p[6]; am.any_ok = (uint8_t *)p[7];
-    am.used = (uint8_t *)p[8];
+    const size_t bn = B * (size_t)am.n * 4, br = B * (size_t)am.ring * 4;
+    DevBufs &ob = h->alarm_bufs;
+    TRY(dev_alloc(h, ob, am.zone_mask, (size_t)am.n_line * 4, d->zone_mask));
     // every instance starts from LinearAttentionBudget.reset: the initial budget, -1 for the times and zones, an empty ring
     const std::vector<float> b0(B, d->init_budget);
-    H2D(am.budget, b0.data(), B * 4);
-    for (int k = 1; k < ALARM_N_BUF - 1; ++k) CU(cudaMemsetAsync(p[k], k <= 4 ? 0xff : 0, sz[k], h->stream));
+    TRY(dev_alloc(h, ob, am.budget, B * 4, b0.data()));
+    TRY(dev_alloc(h, ob, am.time_last, B * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, am.time_last_ok, B * 4, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, am.last, bn, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, am.last_ok, bn, nullptr, 0xff));
+    TRY(dev_alloc(h, ob, am.ring_step, br, nullptr, 0));
+    TRY(dev_alloc(h, ob, am.ring_mask, br, nullptr, 0));
+    TRY(dev_alloc(h, ob, am.any_ok, B, nullptr, 0));
+    TRY(dev_alloc(h, ob, am.used, B, nullptr, 0));
     CU(cudaMemsetAsync(am.illegal, 0, B, h->stream));
     CU(cudaMemsetAsync(am.reward_out, 0, B * 8, h->stream));
     CU(cudaStreamSynchronize(h->stream));
@@ -2551,40 +2452,29 @@ extern "C" int b200pf_alarm_bind(b200pf_handle *h, const b200pf_alarm_desc *d) {
     return 0;
 }
 
-static bool alarm_bound(const b200pf_handle *h) { return env_bound(h) && h->alarm_batch == h->env_batch; }
+// the alarms' per-instance state, in the argument order of b200pf_alarm_get_state / _set_state (the last one, is_alarm_illegal,
+// is the caller's buffer)
+static std::array<StateBuf, 10> alarm_state(const b200pf_handle *h) {
+    const AlarmArgs &am = h->alarm;
+    const size_t B = (size_t)h->alarm_batch, bn = B * (size_t)am.n * 4, br = B * (size_t)am.ring * 4;
+    return {{{am.budget, B * 4}, {am.time_last, B * 4}, {am.time_last_ok, B * 4}, {am.last, bn}, {am.last_ok, bn}, {am.ring_step, br},
+             {am.ring_mask, br}, {am.any_ok, B}, {am.used, B}, {am.illegal, B}}};
+}
 
 extern "C" int b200pf_alarm_get_state(b200pf_handle *h, float *budget, int32_t *time_last, int32_t *time_last_ok, int32_t *last,
                                       int32_t *last_ok, int32_t *ring_step, uint32_t *ring_mask, uint8_t *any_ok, uint8_t *used,
                                       uint8_t *illegal) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!alarm_bound(h)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
-    CU(cudaSetDevice(h->device));
-    size_t sz[ALARM_N_BUF];
-    alarm_sizes(h->alarm.n, h->alarm.ring, (size_t)h->alarm_batch, sz);
-    void *src[ALARM_N_BUF];
-    alarm_buffers(h->alarm, src);
-    void *dst[ALARM_N_BUF] = {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal};
-    CU(cudaStreamSynchronize(h->stream));
-    for (int k = 0; k < ALARM_N_BUF; ++k)
-        if (dst[k]) { CU(cudaMemcpy(dst[k], src[k], sz[k], cudaMemcpyDeviceToHost)); h->env_d2h += (int64_t)sz[k]; }
-    return 0;
+    if (!layer_bound(h, h->alarm_batch)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
+    return state_get(h, alarm_state(h), {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal});
 }
 
 extern "C" int b200pf_alarm_set_state(b200pf_handle *h, const float *budget, const int32_t *time_last, const int32_t *time_last_ok,
                                       const int32_t *last, const int32_t *last_ok, const int32_t *ring_step, const uint32_t *ring_mask,
                                       const uint8_t *any_ok, const uint8_t *used, const uint8_t *illegal) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
-    if (!alarm_bound(h)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
-    CU(cudaSetDevice(h->device));
-    size_t sz[ALARM_N_BUF];
-    alarm_sizes(h->alarm.n, h->alarm.ring, (size_t)h->alarm_batch, sz);
-    void *dst[ALARM_N_BUF];
-    alarm_buffers(h->alarm, dst);
-    const void *src[ALARM_N_BUF] = {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal};
-    for (int k = 0; k < ALARM_N_BUF; ++k)
-        if (src[k]) { H2D(dst[k], src[k], sz[k]); h->env_h2d += (int64_t)sz[k]; }
-    CU(cudaStreamSynchronize(h->stream));
-    return 0;
+    if (!layer_bound(h, h->alarm_batch)) return fail(B200PF_E_STATE, "no alarms bound to the current environment (b200pf_alarm_bind)");
+    return state_set(h, alarm_state(h), {budget, time_last, time_last_ok, last, last_ok, ring_step, ring_mask, any_ok, used, illegal});
 }
 
 extern "C" int b200pf_env_stats(const b200pf_handle *h, int64_t *out8) {

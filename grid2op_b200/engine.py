@@ -11,7 +11,10 @@ from typing import Optional, Tuple
 
 import numpy as np
 
+from .alarm import ALARM_STATE
+from .alert import ALERT_STATE
 from .gridmodel import GridModel
+from .opponent import MULTI_KEYS
 
 __all__ = ["PowerFlowEngine", "PeerBuffer", "EngineUnavailable", "lib_path", "load_library",
            "ST_CONVERGED", "ST_DIVERGED", "ST_UNSUPPLIED", "ST_NO_REF", "ST_TOO_LARGE", "ABI_SYMBOLS"]
@@ -139,11 +142,6 @@ class AlertDesc(C.Structure):
         ("reward_min_no_blackout", C.c_float), ("reward_min_blackout", C.c_float), ("reward_max_no_blackout", C.c_float),
         ("reward_max_blackout", C.c_float), ("raise_alert", C.c_void_p), ("reward_out", C.c_void_p),
     ]
-
-
-# the GeometricOpponentMultiArea's per-instance arrays in the order of b200pf_opp_multi_get_state / _set_state
-_MULTI_STATE = (("multi_mt", np.uint32), ("multi_mt_pos", np.int32), ("multi_wait", np.int32), ("multi_dur", np.int32),
-                ("multi_ctr", np.int32), ("multi_fails", np.int32))
 
 
 def make_env_desc(t: dict, state: dict):
@@ -763,22 +761,30 @@ class PowerFlowEngine:
     def env_reset(self, d_mask: int, d_rows: int = 0):
         self._check(self.lib.b200pf_env_reset(self.h, C.c_void_p(int(d_mask)), C.c_void_p(int(d_rows) or None)), "b200pf_env_reset")
 
+    def _get_state(self, fn: str, spec):
+        """-> {key: array} that the C entry point ``fn`` fills; ``spec``: (key, dtype, shape) in its argument order"""
+        s = {k: np.empty(shape, dt) for k, dt, shape in spec}
+        self._check(getattr(self.lib, fn)(self.h, *[_ptr(s[k]) for k, _, _ in spec]), fn)
+        return s
+
+    def _set_state(self, fn: str, spec, s: dict):
+        """``s[key]`` as ``dtype`` of ``shape`` to the C entry point ``fn`` (None: not copied); ``spec`` as for :meth:`_get_state`"""
+        a = [None if s[k] is None else np.ascontiguousarray(s[k], dt).reshape(shape) for k, dt, shape in spec]
+        self._check(getattr(self.lib, fn)(self.h, *[_ptr(x) for x in a]), fn)
+
     def env_get_state(self):
         """-> dict(topo int8 [B, n_topo_in], t int32 [B], nb_inst int32 [B], cap_dirty bool [B], obs_reset bool [B])"""
-        gm, B = self.gm, self._series_batch
-        topo = np.empty((B, gm.n_topo_in), np.int8); t = np.empty(B, np.int32); nb = np.empty(B, np.int32)
-        cd = np.empty(B, np.uint8); rs = np.empty(B, np.uint8)
-        self._check(self.lib.b200pf_env_get_state(self.h, _ptr(topo), _ptr(t), _ptr(nb), _ptr(cd), _ptr(rs)), "b200pf_env_get_state")
-        return dict(topo=topo, t=t, nb_inst=nb, cap_dirty=cd.astype(bool), obs_reset=rs.astype(bool))
+        B = self._series_batch
+        s = self._get_state("b200pf_env_get_state", (("topo", np.int8, (B, self.gm.n_topo_in)), ("t", np.int32, B), ("nb_inst", np.int32, B),
+                                                      ("cap_dirty", np.uint8, B), ("obs_reset", np.uint8, B)))
+        s["cap_dirty"], s["obs_reset"] = s["cap_dirty"].astype(bool), s["obs_reset"].astype(bool)
+        return s
 
     def env_set_state(self, topo=None, nb_inst=None, cap_dirty=None, obs_reset=None, obs_in=None):
-        gm, B = self.gm, self._series_batch
-        a = None if topo is None else np.ascontiguousarray(topo, np.int8).reshape(B, gm.n_topo_in)
-        b = None if nb_inst is None else np.ascontiguousarray(nb_inst, np.int32)
-        c = None if cap_dirty is None else np.ascontiguousarray(cap_dirty, np.uint8)
-        r = None if obs_reset is None else np.ascontiguousarray(obs_reset, np.uint8)
-        o = None if obs_in is None else np.ascontiguousarray(obs_in, np.int32).reshape(B, -1)
-        self._check(self.lib.b200pf_env_set_state(self.h, _ptr(a), _ptr(b), _ptr(c), _ptr(r), _ptr(o)), "b200pf_env_set_state")
+        B = self._series_batch
+        self._set_state("b200pf_env_set_state", (("topo", np.int8, (B, self.gm.n_topo_in)), ("nb_inst", np.int32, B), ("cap_dirty", np.uint8, B),
+                                                 ("obs_reset", np.uint8, B), ("obs_in", np.int32, (B, -1))),
+                        dict(topo=topo, nb_inst=nb_inst, cap_dirty=cap_dirty, obs_reset=obs_reset, obs_in=obs_in))
 
     def env_pointers(self):
         p = [C.c_void_p() for _ in range(3)]
@@ -797,19 +803,17 @@ class PowerFlowEngine:
         self._check(self.lib.b200pf_opp_bind(self.h, C.byref(d)), "b200pf_opp_bind")
         del keep
 
+    def _opp_spec(self):
+        B = self._series_batch
+        return (("budget", np.float64, B), ("budget64", np.uint8, B), ("ctr", np.int32, (B, 4)), ("mt", np.uint32, (B, 624)),
+                ("mt_pos", np.int32, B))
+
     def opp_get_state(self):
         """-> dict(budget float64 [B], budget64 uint8 [B], ctr int32 [B, 4], mt uint32 [B, 624], mt_pos int32 [B])"""
-        B = self._series_batch
-        s = dict(budget=np.empty(B, np.float64), budget64=np.empty(B, np.uint8), ctr=np.empty((B, 4), np.int32),
-                 mt=np.empty((B, 624), np.uint32), mt_pos=np.empty(B, np.int32))
-        self._check(self.lib.b200pf_opp_get_state(self.h, *[_ptr(s[k]) for k in ("budget", "budget64", "ctr", "mt", "mt_pos")]),
-                    "b200pf_opp_get_state")
-        return s
+        return self._get_state("b200pf_opp_get_state", self._opp_spec())
 
     def opp_set_state(self, s: dict):
-        a = [np.ascontiguousarray(s[k], dt) for k, dt in (("budget", np.float64), ("budget64", np.uint8), ("ctr", np.int32),
-                                                            ("mt", np.uint32), ("mt_pos", np.int32))]
-        self._check(self.lib.b200pf_opp_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_set_state")
+        self._set_state("b200pf_opp_set_state", self._opp_spec(), s)
 
     def opp_geo_bind(self, t: dict):
         """the GeometricOpponent's constants and first schedules (``b200pf_opp_geo_bind``, after ``opp_bind`` with kind 3): ``t``
@@ -826,17 +830,16 @@ class PowerFlowEngine:
         self._opp_geo_cap = cap
         del keep
 
+    def _opp_geo_spec(self):
+        B, cap = self._series_batch, getattr(self, "_opp_geo_cap", 0)       # (unbound: the library refuses the call)
+        return (("geo_wait", np.int32, (B, cap)), ("geo_dur", np.int32, (B, cap)), ("geo_ctr", np.int32, (B, 4)))
+
     def opp_geo_get_state(self):
         """-> dict(geo_wait int32 [B, cap], geo_dur int32 [B, cap], geo_ctr int32 [B, 4]) of the GeometricOpponent"""
-        B, cap = self._series_batch, getattr(self, "_opp_geo_cap", 0)       # (unbound: the library refuses the call)
-        s = dict(geo_wait=np.empty((B, cap), np.int32), geo_dur=np.empty((B, cap), np.int32), geo_ctr=np.empty((B, 4), np.int32))
-        self._check(self.lib.b200pf_opp_geo_get_state(self.h, *[_ptr(s[k]) for k in ("geo_wait", "geo_dur", "geo_ctr")]),
-                    "b200pf_opp_geo_get_state")
-        return s
+        return self._get_state("b200pf_opp_geo_get_state", self._opp_geo_spec())
 
     def opp_geo_set_state(self, s: dict):
-        a = [np.ascontiguousarray(s[k], np.int32) for k in ("geo_wait", "geo_dur", "geo_ctr")]
-        self._check(self.lib.b200pf_opp_geo_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_geo_set_state")
+        self._set_state("b200pf_opp_geo_set_state", self._opp_geo_spec(), s)
 
     def opp_multi_bind(self, t: dict, d_attack_lines: int):
         """the GeometricOpponentMultiArea's areas, constants and first state (``b200pf_opp_multi_bind``, after ``opp_bind`` with kind
@@ -844,7 +847,7 @@ class PowerFlowEngine:
         int32 [B, n_area] for each step's attacked lines"""
         keep = dict(area_off=np.ascontiguousarray(t["area_off"], np.int32), weights=np.ascontiguousarray(t["weights"], np.float64),
                     emt=np.ascontiguousarray(t["episode_max_time"], np.int32))
-        keep.update({k: np.ascontiguousarray(t[k], dt) for k, dt in _MULTI_STATE})
+        keep.update({k: np.ascontiguousarray(t[k], dt) for k, dt, _ in self._opp_multi_spec()})
         n_area, cap = int(keep["multi_wait"].shape[1]), int(keep["multi_wait"].shape[2])
         d = OppMultiDesc(n_area=n_area, area_off=keep["area_off"].ctypes.data, weights=keep["weights"].ctypes.data,
                          p_hazard=float(t["p_hazard"]), p_recovery=float(t["p_recovery"]), logq_hazard=float(t["logq_hazard"]),
@@ -856,20 +859,18 @@ class PowerFlowEngine:
         self._opp_multi_shape = (n_area, cap)
         del keep
 
+    def _opp_multi_spec(self):
+        B = self._series_batch
+        A, cap = getattr(self, "_opp_multi_shape", (0, 0))                   # (unbound: the library refuses the call)
+        return tuple(zip(MULTI_KEYS, (np.uint32,) + (np.int32,) * 5, ((B, A, 624), (B, A), (B, A, cap), (B, A, cap), (B, A, 6), (B,))))
+
     def opp_multi_get_state(self):
         """-> dict(multi_mt uint32 [B, n_area, 624], multi_mt_pos int32 [B, n_area], multi_wait / multi_dur int32 [B, n_area, cap],
         multi_ctr int32 [B, n_area, 6], multi_fails int32 [B]) of the GeometricOpponentMultiArea"""
-        B = self._series_batch
-        A, cap = getattr(self, "_opp_multi_shape", (0, 0))                   # (unbound: the library refuses the call)
-        shapes = dict(multi_mt=(B, A, 624), multi_mt_pos=(B, A), multi_wait=(B, A, cap), multi_dur=(B, A, cap), multi_ctr=(B, A, 6),
-                      multi_fails=(B,))
-        s = {k: np.empty(shapes[k], dt) for k, dt in _MULTI_STATE}
-        self._check(self.lib.b200pf_opp_multi_get_state(self.h, *[_ptr(s[k]) for k, _ in _MULTI_STATE]), "b200pf_opp_multi_get_state")
-        return s
+        return self._get_state("b200pf_opp_multi_get_state", self._opp_multi_spec())
 
     def opp_multi_set_state(self, s: dict):
-        a = [np.ascontiguousarray(s[k], dt) for k, dt in _MULTI_STATE]
-        self._check(self.lib.b200pf_opp_multi_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_opp_multi_set_state")
+        self._set_state("b200pf_opp_multi_set_state", self._opp_multi_spec(), s)
 
     def alert_bind(self, a, d_raise: int, d_reward: int):
         """line alerts of the device environment (``b200pf_alert_bind``): ``a`` a :class:`grid2op_b200.alert.BatchedAlerts` (lines,
@@ -883,20 +884,18 @@ class PowerFlowEngine:
         self._check(self.lib.b200pf_alert_bind(self.h, C.byref(d)), "b200pf_alert_bind")
         self._alert_shape = (len(lines), int(a.ring))
 
-    def alert_get_state(self):
-        """-> the alert state of every instance, the arrays of :data:`grid2op_b200.alert.ALERT_STATE`"""
-        from .alert import ALERT_STATE
+    def _alert_spec(self):
         B = self._series_batch
         n, R = getattr(self, "_alert_shape", (0, 0))                        # (unbound: the library refuses the call)
-        s = {k: np.empty((B,) if k in ("total", "cur_id") else (B, R, n) if k in ("ts_attack", "launched") else (B, n), dt)
-             for k, dt in ALERT_STATE}
-        self._check(self.lib.b200pf_alert_get_state(self.h, *[_ptr(s[k]) for k, _ in ALERT_STATE]), "b200pf_alert_get_state")
-        return s
+        return tuple((k, dt, (B,) if k in ("total", "cur_id") else (B, R, n) if k in ("ts_attack", "launched") else (B, n))
+                     for k, dt in ALERT_STATE)
+
+    def alert_get_state(self):
+        """-> the alert state of every instance, the arrays of :data:`grid2op_b200.alert.ALERT_STATE`"""
+        return self._get_state("b200pf_alert_get_state", self._alert_spec())
 
     def alert_set_state(self, s: dict):
-        from .alert import ALERT_STATE
-        a = [np.ascontiguousarray(s[k], dt) for k, dt in ALERT_STATE]
-        self._check(self.lib.b200pf_alert_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_alert_set_state")
+        self._set_state("b200pf_alert_set_state", self._alert_spec(), s)
 
     def alarm_bind(self, a, d_raise: int, d_reward: int, d_illegal: int):
         """alarms of the device environment (``b200pf_alarm_bind``): ``a`` a :class:`grid2op_b200.alarm.BatchedAlarms` (zones,
@@ -910,20 +909,18 @@ class PowerFlowEngine:
         self._check(self.lib.b200pf_alarm_bind(self.h, C.byref(d)), "b200pf_alarm_bind")
         self._alarm_shape = (int(a.n), int(a.ring))
 
-    def alarm_get_state(self):
-        """-> the alarm state of every instance, the arrays of :data:`grid2op_b200.alarm.ALARM_STATE`"""
-        from .alarm import ALARM_STATE
+    def _alarm_spec(self):
         B = self._series_batch
         n, R = getattr(self, "_alarm_shape", (0, 0))                        # (unbound: the library refuses the call)
         shapes = dict(last=(B, n), last_ok=(B, n), ring_step=(B, R), ring_mask=(B, R))
-        s = {k: np.empty(shapes.get(k, (B,)), dt) for k, dt in ALARM_STATE}
-        self._check(self.lib.b200pf_alarm_get_state(self.h, *[_ptr(s[k]) for k, _ in ALARM_STATE]), "b200pf_alarm_get_state")
-        return s
+        return tuple((k, dt, shapes.get(k, (B,))) for k, dt in ALARM_STATE)
+
+    def alarm_get_state(self):
+        """-> the alarm state of every instance, the arrays of :data:`grid2op_b200.alarm.ALARM_STATE`"""
+        return self._get_state("b200pf_alarm_get_state", self._alarm_spec())
 
     def alarm_set_state(self, s: dict):
-        from .alarm import ALARM_STATE
-        a = [np.ascontiguousarray(s[k], dt) for k, dt in ALARM_STATE]
-        self._check(self.lib.b200pf_alarm_set_state(self.h, *[_ptr(x) for x in a]), "b200pf_alarm_set_state")
+        self._set_state("b200pf_alarm_set_state", self._alarm_spec(), s)
 
     def observe_device(self, d_obs: int, d_reward: int = 0):
         self._check(self.lib.b200pf_observe_device(self.h, C.c_void_p(d_obs), C.c_void_p(d_reward or None)), "b200pf_observe_device")
