@@ -4,11 +4,13 @@ topology agent depends on.
 
 What one :meth:`BatchedEnv.step` restates for a whole batch of independent environments (reference, per env —
 ``BaseEnv.step`` grid2op/Environment/baseEnv.py:3778-3872 and what it calls), for the action subset
-{do nothing, set the busbars of ONE substation, set the status of ONE line} (``MAX_SUB_CHANGED = MAX_LINE_STATUS_CHANGED
-= 1``, grid2op/Parameters.py:279):
+{do nothing, set the busbars of ONE substation, set the status of ONE line} (the ``sub_id`` / ``line_id`` arguments), or
+grid2op's native topology action (``set_bus`` / ``change_bus`` / ``set_line_status`` / ``change_line_status`` vectors,
+:meth:`BatchedEnv._apply_actions`):
 
-1. legality — ``DefaultRules``: an action that touches a line whose ``times_before_line_status_actionable`` is > 0 or a
-   substation whose ``times_before_topology_actionable`` is > 0 is illegal and replaced by "do nothing"
+1. legality — ``LookParam`` (``max_sub_changed`` / ``max_line_status_changed``, grid2op/Parameters.py:279; or the same maxima per
+   area of ``RulesByArea``) and ``PreventReconnection``: an action that touches a line whose ``times_before_line_status_actionable``
+   is > 0 or a substation whose ``times_before_topology_actionable`` is > 0 is illegal and replaced by "do nothing"
    (grid2op/Rules/PreventReconnection.py:33-60, baseEnv.py:3798-3820);
 2. ``_backend_action += action`` (baseEnv.py:3822-3846): busbars of the substation's elements, line disconnection
    (both ends -1) / reconnection (each end back on its last busbar, grid2op/Action/_backendAction.py ``last_topo_registered``);
@@ -42,10 +44,16 @@ __all__ = ["BatchedEnv", "random_substation_actions"]
 class BatchedEnv(BatchedDoNothing):
     def __init__(self, gm: GridModel, chron: np.ndarray, batch: int, *, maintenance: Optional[np.ndarray] = None,
                  hazards: Optional[np.ndarray] = None, nb_timestep_cooldown_line: int = 0, nb_timestep_cooldown_sub: int = 0,
-                 nb_timestep_reconnection: int = 10, engine=None, tight_cap: bool = True, **kw):
+                 nb_timestep_reconnection: int = 10, engine=None, tight_cap: bool = True, max_sub_changed: int = 1,
+                 max_line_status_changed: int = 1, rules_by_area=None, **kw):
         """``maintenance`` / ``hazards``: bool [n_scen, n_rows, n_line] (:func:`grid2op_b200.chronics.load_line_events` per
         scenario), row-aligned with ``chron``.  Cooldown parameters: grid2op.Parameters NB_TIMESTEP_COOLDOWN_LINE /
-        NB_TIMESTEP_COOLDOWN_SUB / NB_TIMESTEP_RECONNECTION (Parameters.py:255-300)."""
+        NB_TIMESTEP_COOLDOWN_SUB / NB_TIMESTEP_RECONNECTION (Parameters.py:255-300).  Legality: ``max_sub_changed`` /
+        ``max_line_status_changed`` are MAX_SUB_CHANGED / MAX_LINE_STATUS_CHANGED; ``rules_by_area``, a list of lists of substation
+        ids as ``RulesByArea(areas_list)`` takes them, applies these maxima per area instead of over the whole grid (at most 16
+        areas).  Without it the rules are ``LookParam`` + ``PreventReconnection`` (``DefaultRules`` at the default maxima)."""
+        if int(max_sub_changed) < 0 or int(max_line_status_changed) < 0:
+            raise ValueError("max_sub_changed and max_line_status_changed must be >= 0")
         super().__init__(gm, chron, batch, engine=engine, **kw)
         B, nl = self.batch, gm.n_line
         self.topo = self.topo0.copy()                                      # int8 [B, n_topo_in], -1 = disconnected
@@ -85,6 +93,10 @@ class BatchedEnv(BatchedDoNothing):
         self.line_of_pos[self.line_or_pos] = np.arange(nl); self.line_of_pos[self.line_ex_pos] = np.arange(nl)
         self.other_end_pos[self.line_or_pos] = self.line_ex_pos; self.other_end_pos[self.line_ex_pos] = self.line_or_pos
         self._topo_dirty = False
+        self.max_sub_changed, self.max_line_status_changed = int(max_sub_changed), int(max_line_status_changed)
+        self._set_rules_by_area(rules_by_area)
+        self._pos_sub = np.zeros((gm.dim_topo, gm.n_sub), dtype=np.int64)             # one-hot substation of each position
+        self._pos_sub[np.arange(gm.dim_topo), sub_of] = 1
         # Shunts: this driver never acts on them, so the environment of the reference holds every shunt for connected to busbar 1
         # (_BackendAction.current_shunt_bus, grid2op/Action/_backendAction.py:513-514) and counts that busbar as active
         # (:1519-1531 -> bus.in_service, pandaPowerBackend.py:920-922) — also when the grid file has the shunt out of service (all six of
@@ -105,6 +117,7 @@ class BatchedEnv(BatchedDoNothing):
         self.n_illegal = 0
         self.n_steps = 0
         self.is_illegal = np.zeros(B, dtype=bool)                          # the last step's action was replaced by "do nothing"
+        self.is_ambiguous = np.zeros(B, dtype=bool)                        # ... as ambiguous (the vector action)
         self.current_step = np.zeros(B, dtype=np.int32)                    # env.nb_time_step (obs.current_step)
         self.soft_overflow_threshold = float(kw.get("soft_overflow_threshold", 1.0))
         self._obs = None
@@ -117,6 +130,46 @@ class BatchedEnv(BatchedDoNothing):
         self._alarms = None                                                # alarms (:meth:`enable_alarms`)
 
     # ------------------------------------------------------------------------------------------------------------
+    def _set_rules_by_area(self, areas):
+        """``RulesByArea.__init__`` + ``initialize`` (grid2op/Rules/rulesByArea.py): each area's substations sorted and de-duplicated,
+        as many listed as the grid has (ValueError where grid2op raises Grid2OpException), a line in the area of its origin
+        substation.  -> ``self.areas`` (None or the areas' substation ids), ``self.lines_id_by_area``, the area masks ``_sub_area`` /
+        ``_line_area`` (uint32, bit k: area k) and the membership matrices the counts use (one area of everything without areas)."""
+        gm = self.gm
+        self.areas = self.lines_id_by_area = self._sub_area = self._line_area = None
+        if areas is None:
+            self._sub_area_mat = np.ones((gm.n_sub, 1), dtype=np.int64)
+            self._line_area_mat = np.ones((gm.n_line, 1), dtype=np.int64)
+            return
+        areas = [np.unique(np.asarray(list(a), dtype=np.int64)) for a in areas]
+        if not 1 <= len(areas) <= 16:
+            raise ValueError(f"{len(areas)} areas, 1 to 16 supported")
+        if sum(len(a) for a in areas) != gm.n_sub:
+            raise ValueError(f"the areas list {sum(len(a) for a in areas)} substations, the grid has {gm.n_sub}")
+        if any(((a < 0) | (a >= gm.n_sub)).any() for a in areas):
+            raise ValueError("substation id out of range in rules_by_area")
+        line_or_sub = np.asarray(gm.line_or_sub, dtype=np.int64)
+        self.areas = areas
+        self.lines_id_by_area = [np.flatnonzero(np.isin(line_or_sub, a)) for a in areas]
+        self._sub_area_mat = np.zeros((gm.n_sub, len(areas)), dtype=np.int64)
+        self._line_area_mat = np.zeros((gm.n_line, len(areas)), dtype=np.int64)
+        for k, (a, l) in enumerate(zip(areas, self.lines_id_by_area)):
+            self._sub_area_mat[a, k] = 1
+            self._line_area_mat[l, k] = 1
+        w = np.left_shift(np.uint32(1), np.arange(len(areas), dtype=np.uint32))
+        self._sub_area = (self._sub_area_mat.astype(np.uint32) * w).sum(axis=1).astype(np.uint32)
+        self._line_area = (self._line_area_mat.astype(np.uint32) * w).sum(axis=1).astype(np.uint32)
+
+    def _illegal(self, aff_l, aff_s) -> np.ndarray:
+        """bool [B]: the legality rules on an action's topological impact, ``aff_l`` [B, n_line] / ``aff_s`` [B, n_sub] (counts or
+        bools): LookParam's maxima over the whole grid or RulesByArea._lookparam_byarea's per area, and PreventReconnection (an
+        impacted line or substation in cooldown), grid2op/Rules/LookParam.py, rulesByArea.py, PreventReconnection.py:33-60"""
+        aff_l, aff_s = np.asarray(aff_l, dtype=np.int64), np.asarray(aff_s, dtype=np.int64)
+        bad = ((aff_l @ self._line_area_mat) > self.max_line_status_changed).any(axis=1)
+        bad |= ((aff_s @ self._sub_area_mat) > self.max_sub_changed).any(axis=1)
+        bad |= ((aff_l > 0) & (self.line_cooldown > 0)).any(axis=1) | ((aff_s > 0) & (self.sub_cooldown > 0)).any(axis=1)
+        return bad
+
     def _bus_cap(self) -> int:
         """Active buses (bus slots with a connected element) of the fullest instance, rounded up to a multiple of 8 above 17
         (<= 17: exact — the warp-per-instance kernel takes systems up to 17 buses), at most every bus slot.  Per-instance counts are
@@ -143,7 +196,6 @@ class BatchedEnv(BatchedDoNothing):
         gm, B = self.gm, self.batch
         aff_l = np.zeros((B, gm.n_line), dtype=bool)
         aff_s = np.zeros((B, gm.n_sub), dtype=bool)
-        idx = np.arange(B)
         has_sub = np.zeros(B, dtype=bool)
         has_line = np.zeros(B, dtype=bool)
         if sub_id is not None:
@@ -159,8 +211,8 @@ class BatchedEnv(BatchedDoNothing):
         # _BackendAction: the other end goes back to its last busbar)
         reco = None
         sub_impacted = has_sub.copy()
-        n_reco = np.zeros(B, dtype=np.int64)
-        reco_in_cd = np.zeros(B, dtype=bool)
+        cnt_l = np.zeros((B, gm.n_line), dtype=np.int64)  # impacted lines (each reconnecting entry counts once) and substations
+        cnt_s = np.zeros((B, gm.n_sub), dtype=np.int64)
         reco_is_line = np.zeros(B, dtype=bool)           # the explicitly named line is one of the reconnected ones
         if has_sub.any():
             who_s = np.flatnonzero(has_sub)
@@ -177,24 +229,20 @@ class BatchedEnv(BatchedDoNothing):
                 lp = np.where(pos >= 0, self.line_of_pos[psafe], -1)
                 reco = dead & (lp >= 0)
                 if reco.any():
-                    lsafe = np.where(lp >= 0, lp, 0)
-                    n_reco[who_s] = reco.sum(axis=1)
-                    reco_in_cd[who_s] = (reco & (self.line_cooldown[who_s[:, None], lsafe] > 0)).any(axis=1)
+                    np.add.at(cnt_l, (np.broadcast_to(who_s[:, None], pos.shape)[reco], lp[reco]), 1)
                     if line_id is not None:
                         reco_is_line[who_s] = (reco & (lp == np.where(has_line[who_s], line_id[who_s], -2)[:, None])).any(axis=1)
                     sub_impacted[who_s] = (m & ~reco).any(axis=1)
                 else:
                     reco = None
-        # legality (DefaultRules: LookParam MAX_SUB_CHANGED = MAX_LINE_STATUS_CHANGED = 1, grid2op/Rules/LookParam.py; PreventReconnection on
-        # what the action impacts, grid2op/Rules/PreventReconnection.py:33-60); finished instances ignore their action
-        illegal = np.zeros(B, dtype=bool)
-        if has_sub.any():
-            illegal |= sub_impacted & (self.sub_cooldown[idx, np.where(has_sub, sub_id, 0)] > 0)
-            if reco is not None:
-                illegal |= reco_in_cd
-                illegal |= (n_reco + (has_line & ~reco_is_line)) > 1
-        if has_line.any():
-            illegal |= has_line & (self.line_cooldown[idx, np.where(has_line, line_id, 0)] > 0)
+        # legality (:meth:`_illegal`) on what the action impacts; finished instances ignore their action
+        if sub_id is not None:
+            w = np.flatnonzero(has_sub & sub_impacted)
+            cnt_s[w, sub_id[w]] = 1
+        if line_id is not None:
+            w = np.flatnonzero(has_line & ~reco_is_line)
+            cnt_l[w, line_id[w]] += 1
+        illegal = self._illegal(cnt_l, cnt_s)
         self.n_illegal += int((illegal & ~self.done).sum())
         self.is_illegal = illegal & ~self.done
         ok = ~illegal & ~self.done
@@ -233,6 +281,103 @@ class BatchedEnv(BatchedDoNothing):
                 self._cap_dirty[who] = True
         return aff_l, aff_s
 
+    def _apply_actions(self, sb, cb, ss, cs):
+        """grid2op's native topology action (``set_bus`` int [B, dim_topo], ``change_bus`` bool [B, dim_topo], ``set_line_status`` int
+        [B, n_line], ``change_line_status`` bool [B, n_line], checked by :meth:`_vector_action`) in BaseEnv.step's order
+        (baseEnv.py:3706-3767): BaseAction's topology ambiguity (baseAction.py:3558-3565, :3670-3771), the topological impact on the
+        line status the previous step left (:1796-2022), legality (:meth:`_illegal`), and _BackendAction.__iadd__'s application
+        (_backendAction.py:738-765, :810-919) with the busbars last registered.  A disconnected end is one <= 0.
+        -> (aff_lines bool [B, n_line], aff_subs bool [B, n_sub]) of the LEGAL actions, applied to self.topo"""
+        self._to_host()
+        gm = self.gm
+        lor, lex = self.line_or_pos, self.line_ex_pos
+        live = ~self.done
+        so, se = sb[:, lor], sb[:, lex]
+        ch = cb[:, lor] | cb[:, lex]
+        amb = ((sb != 0) & cb).any(axis=1) | ((ss != 0) & cs).any(axis=1)
+        amb |= (((so == -1) & (se > 0)) | ((se == -1) & (so > 0))).any(axis=1)
+        amb |= ((ss == -1) & ((so > 0) | (se > 0) | ch)).any(axis=1)
+        amb |= ((ss == 1) & ((so == -1) | (se == -1) | ch)).any(axis=1)
+        amb &= live
+        # the impact: lines whose status is set, changed or reached through one end's busbar; substations of the other bus changes
+        on = (self.topo[:, lor] > 0) & (self.topo[:, lex] > 0)
+        named = cs | (ss != 0)
+        conn = ((so > 0) | (se > 0)) & ~on
+        disc = ((so < 0) | (se < 0)) & on
+        aff_l = named | conn | disc
+        clear = (named & ~on) | conn | disc
+        eff = cb | (sb != 0)
+        eff[:, lor] &= ~clear
+        eff[:, lex] &= ~clear
+        aff_s = (eff.astype(np.int64) @ self._pos_sub) > 0
+        illegal = ~amb & self._illegal(aff_l, aff_s)
+        self.is_illegal = illegal & live
+        self.n_illegal += int(self.is_illegal.sum())
+        self.is_ambiguous = amb
+        ok = live & ~amb & ~illegal
+        aff_l &= ok[:, None]
+        aff_s &= ok[:, None]
+        w = np.flatnonzero(ok & ((sb != 0).any(axis=1) | cb.any(axis=1) | (ss != 0).any(axis=1) | cs.any(axis=1)))
+        if not len(w):
+            return aff_l, aff_s
+
+        def topo_stage(v, c, s):                                             # change_bus (connected: 1 <-> 2), then set_bus
+            v = np.where(c & (v > 0), 3 - v, v)
+            return np.where(s != 0, s, v)
+
+        nt = gm.dim_topo
+        t = self.topo[w, :nt].astype(np.int64)
+        lb = self.last_bus[w].astype(np.int64)
+        sbw, cbw, ssw, csw = sb[w].astype(np.int64), cb[w], ss[w], cs[w]
+        lbo, lbe = lb[:, lor], lb[:, lex]
+        vo, ve = t[:, lor], t[:, lex]
+        was = (vo > 0) | (ve > 0)                                            # change_status, then set_status
+        vo, ve = np.where(csw, np.where(was, -1, lbo), vo), np.where(csw, np.where(was, -1, lbe), ve)
+        vo = np.where(ssw < 0, -1, np.where((ssw > 0) & (vo <= 0), lbo, vo))
+        ve = np.where(ssw < 0, -1, np.where((ssw > 0) & (ve <= 0), lbe, ve))
+        before_off = vo <= 0                                                 # _status_or_before
+        disco = before_off | (ve <= 0)
+        vo, ve = topo_stage(vo, cbw[:, lor], sbw[:, lor]), topo_stage(ve, cbw[:, lex], sbw[:, lex])
+        reco = before_off & ((vo > 0) | (ve > 0))                            # _aux_iadd_reconcile_disco_reco
+        off = ~reco & (disco | (vo <= 0) | (ve <= 0))
+        vo = np.where(reco & (vo <= 0), lbo, np.where(off, -1, vo))
+        ve = np.where(reco & (ve <= 0), lbe, np.where(off, -1, ve))
+        t = topo_stage(t, cbw, sbw)
+        t[:, lor], t[:, lex] = vo, ve
+        self.topo[w, :nt] = t
+        self.last_bus[w] = np.where(t > 0, t, lb)                            # last_topo_registered.update_connected
+        self._topo_dirty = True
+        self._cap_dirty[w] = True
+        return aff_l, aff_s
+
+    def _vector_action(self, set_bus, change_bus, set_line_status, change_line_status):
+        """the four vectors of :meth:`step` checked and completed with zeros -> (set_bus int8 [B, dim_topo], change_bus bool
+        [B, dim_topo], set_line_status int8 [B, n_line], change_line_status bool [B, n_line]), or None when none is given"""
+        if set_bus is None and change_bus is None and set_line_status is None and change_line_status is None:
+            return None
+        gm, B = self.gm, self.batch
+        out = []
+        for x, name, n, kinds in ((set_bus, "set_bus", gm.dim_topo, "iu"), (change_bus, "change_bus", gm.dim_topo, "b"),
+                                  (set_line_status, "set_line_status", gm.n_line, "iu"),
+                                  (change_line_status, "change_line_status", gm.n_line, "b")):
+            if x is None:
+                out.append(np.zeros((B, n), dtype=bool if kinds == "b" else np.int8))
+                continue
+            x = np.asarray(x)
+            if x.shape != (B, n) or x.dtype.kind not in kinds:
+                raise ValueError(f"{name} must be a {'bool' if kinds == 'b' else 'int8'} array of shape {(B, n)}")
+            out.append(x.astype(bool) if kinds == "b" else x)
+        sb, cb, ss, cs = out
+        if ((sb < -1) | (sb > gm.n_busbar)).any():
+            raise ValueError(f"set_bus outside [-1, {gm.n_busbar}]")
+        if ((sb == -1) & (self.line_of_pos < 0)[None, :]).any():
+            raise ValueError("set_bus = -1 on a load, generator or storage unit (detachment is not supported)")
+        if cb.any() and gm.n_busbar != 2:
+            raise ValueError("change_bus needs two busbars per substation")
+        if ((ss < -1) | (ss > 1)).any():
+            raise ValueError("set_line_status outside {-1, 0, 1}")
+        return sb.astype(np.int8), cb, ss.astype(np.int8), cs
+
     def _isolated_shunt_busbar(self) -> np.ndarray:
         """bool [B]: busbar 1 of a substation whose shunt is out of service in the grid file carries no element any more — for the
         reference an in-service bus without a voltage: ``runpf`` fails with "Isolated bus" (pandaPowerBackend.py:1241-1244) and the
@@ -270,12 +415,22 @@ class BatchedEnv(BatchedDoNothing):
                 self._cap_dirty[ii[was_on]] = True
 
     def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
-             raise_alarm=None):
+             raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None):
         """One env.step of every instance.  ``sub_id`` int [B] (-1: none) with ``sub_bus`` int8 [B, >= max_sub_size] (busbar per
         element of that substation in topology-vector order, 0 = leave); ``line_id`` int [B] (-1: none) with ``line_status``
         int [B] (+1 reconnect / -1 disconnect); ``raise_alert`` bool [B, dim_alerts] (:meth:`enable_alerts`; None: no alert,
         ignored on a reset step); ``raise_alarm`` bool [B, dim_alarms] (:meth:`enable_alarms`; None: no alarm, ignored on a reset
-        step).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the device (:meth:`fetch`)."""
+        step).  Returns ``(rho [B, n_line], done [B], info)``; the full records stay on the device (:meth:`fetch`).
+
+        grid2op's native topology action instead of the ``sub_id`` / ``line_id`` pair (any subset of the four, not together with
+        that pair): ``set_bus`` int8 [B, dim_topo] in ``topo_vect`` order (0 leave, -1 disconnect a line end, 1..n_busbar),
+        ``change_bus`` bool [B, dim_topo] (two busbars per substation only), ``set_line_status`` int8 [B, n_line] in {-1, 0, 1},
+        ``change_line_status`` bool [B, n_line]; :meth:`_apply_actions` restates what grid2op does with them.  ``info["is_ambiguous"]``
+        (bool [B]) then says which actions were replaced by "do nothing" as ambiguous.  A value out of range, ``set_bus = -1`` on a
+        load, generator or storage unit, a wrong shape or dtype raise ValueError and change nothing."""
+        vec = self._vector_action(set_bus, change_bus, set_line_status, change_line_status)
+        if vec is not None and (sub_id is not None or line_id is not None):
+            raise ValueError("the vector action (set_bus, change_bus, set_line_status, change_line_status) replaces sub_id / line_id")
         if raise_alert is not None:
             if self._alerts is None:
                 raise ValueError("raise_alert without enable_alerts()")
@@ -295,8 +450,13 @@ class BatchedEnv(BatchedDoNothing):
         opp = None
         if self._opp is not None:             # the opponent decides on the line status and rho the previous step left
             opp = self._opponent_decide(from_reset)
-        aff_l, aff_s = self._apply_agent(sub_id, sub_bus, line_id, line_status) if not from_reset else (
-            np.zeros((self.batch, gm.n_line), dtype=bool), np.zeros((self.batch, gm.n_sub), dtype=bool))
+        self.is_ambiguous = np.zeros(self.batch, dtype=bool)
+        if from_reset:
+            aff_l, aff_s = np.zeros((self.batch, gm.n_line), dtype=bool), np.zeros((self.batch, gm.n_sub), dtype=bool)
+        elif vec is not None:
+            aff_l, aff_s = self._apply_actions(*vec)
+        else:
+            aff_l, aff_s = self._apply_agent(sub_id, sub_bus, line_id, line_status)
         self._apply_environment()
         if opp is not None:                   # its attack lands after the agent's action and the environment's outages
             self._apply_attack(*opp)
@@ -362,9 +522,11 @@ class BatchedEnv(BatchedDoNothing):
             self.current_step[live] += 1
         alarm_reward = None
         if self._alarms is not None:          # registered once the step's legality is known; an instance finished before keeps its state
-            alarm_reward = self._alarms.step(None if from_reset else raise_alarm, live & (not from_reset), self.is_illegal,
+            alarm_reward = self._alarms.step(None if from_reset else raise_alarm, live & (not from_reset), self.is_illegal | self.is_ambiguous,
                                              self.current_step, newly_done, disc).copy()
         info = {"status": status, "iters": iters, "disc_lines": disc, "newly_done": newly_done, "is_illegal": self.is_illegal.copy()}
+        if vec is not None:
+            info["is_ambiguous"] = self.is_ambiguous.copy()
         if opp is not None:
             info["opponent_attack_line"], info["opponent_attack_duration"] = opp
         if alert_reward is not None and self._alerts.reward:
@@ -617,7 +779,7 @@ class BatchedEnv(BatchedDoNothing):
         self.last_bus[idx] = np.where(self.topo0[idx, :self.gm.dim_topo] > 0, self.topo0[idx, :self.gm.dim_topo], 1)
         self.line_cooldown[idx] = 0; self.sub_cooldown[idx] = 0
         self.done[idx] = False
-        self.current_step[idx] = 0; self.is_illegal[idx] = False
+        self.current_step[idx] = 0; self.is_illegal[idx] = False; self.is_ambiguous[idx] = False
         if self._obs is not None:
             self._obs["reset"][idx] = True
         self.row[idx] = rows
@@ -671,7 +833,7 @@ class BatchedEnv(BatchedDoNothing):
 
     def observe_inputs(self) -> np.ndarray:
         """int32 [B, n_line + n_sub + 3]: the per-instance values only the host knows (cooldowns, current_step, step stamp, flags
-        illegal / game over / reset) — what one observe launch copies to the device; with alerts, 6 dim_alerts + 1 more columns
+        illegal / game over / reset / ambiguous) — what one observe launch copies to the device; with alerts, 6 dim_alerts + 1 more columns
         (the alert values, :meth:`grid2op_b200.alert.BatchedAlerts.obs_record`); with alarms, dim_alarms + 4 more (the alarm values,
         :meth:`grid2op_b200.alarm.BatchedAlarms.obs_record`)."""
         self._to_host()
@@ -680,7 +842,7 @@ class BatchedEnv(BatchedDoNothing):
         nl, ns = gm.n_line, gm.n_sub
         h[:, :nl] = self.line_cooldown; h[:, nl:nl + ns] = self.sub_cooldown
         h[:, nl + ns] = self.current_step; h[:, nl + ns + 1] = self.n_steps
-        h[:, nl + ns + 2] = self.is_illegal * 1 + self.done * 2 + o["reset"] * 4
+        h[:, nl + ns + 2] = self.is_illegal * 1 + self.done * 2 + o["reset"] * 4 + self.is_ambiguous * 8
         if self._alerts is not None:
             h[:, nl + ns + 3:nl + ns + 4 + 6 * self._alerts.n] = self._alerts.obs_record()
         if self._alarms is not None:
@@ -753,14 +915,21 @@ class BatchedEnv(BatchedDoNothing):
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)       # noqa: E731
         st = dict(last_bus=z((B, gm.dim_topo), torch.int8), line_cd=z((B, gm.n_line), torch.int32), sub_cd=z((B, gm.n_sub), torch.int32),
                   done=z(B, torch.bool), is_illegal=z(B, torch.bool), newly_done=z(B, torch.bool), current_step=z(B, torch.int32),
-                  status=z(B, torch.int32))
+                  status=z(B, torch.int32), is_ambiguous=z(B, torch.bool))
         if self._iso_cols is None:
             self._isolated_shunt_busbar()                 # (builds the column segments)
         tables = dict(sub_pos=self.sub_pos, line_of_pos=self.line_of_pos, other_end_pos=self.other_end_pos, cd_line=self.cd_line,
                       cd_sub=self.cd_sub, cd_reco=self.cd_reco, maint=self._maint, haz=self._haz, maint_time=self._maint_time,
                       maint_dur=self._maint_dur, haz_dur=self._haz_dur, iso_seg=self._iso_seg, iso_cols=self._iso_cols,
                       topo0=self.topo0, t0=self.t0)
-        self.engine.env_bind(tables, {k: v.data_ptr() for k, v in st.items()})
+        self.engine.env_bind(tables, {k: v.data_ptr() for k, v in st.items() if k != "is_ambiguous"})
+        # the rules, and the vector action's buffers: step_tensors copies the caller's tensors into them on the device
+        st.update(act_set_bus=z((B, gm.dim_topo), torch.int8), act_change_bus=z((B, gm.dim_topo), torch.bool),
+                  act_set_status=z((B, gm.n_line), torch.int8), act_change_status=z((B, gm.n_line), torch.bool))
+        self.engine.act_bind(self.max_sub_changed, self.max_line_status_changed, 0 if self.areas is None else len(self.areas),
+                             self._sub_area, self._line_area,
+                             st["act_set_bus"].data_ptr(), st["act_change_bus"].data_ptr(), st["act_set_status"].data_ptr(),
+                             st["act_change_status"].data_ptr(), st["is_ambiguous"].data_ptr())
         p, q = self.engine.series_device_pointers(), self.engine.env_pointers()
         st["rho"] = _device_view(p["rho"], (B, gm.n_line), "<f4", dev)
         st["iters"] = _device_view(p["iters"], (B,), "<i4", dev)
@@ -827,7 +996,7 @@ class BatchedEnv(BatchedDoNothing):
         if self._authority == "device":
             return
         for name, arr in (("last_bus", self.last_bus), ("line_cd", self.line_cooldown), ("sub_cd", self.sub_cooldown), ("done", self.done),
-                          ("is_illegal", self.is_illegal), ("current_step", self.current_step)):
+                          ("is_illegal", self.is_illegal), ("current_step", self.current_step), ("is_ambiguous", self.is_ambiguous)):
             d[name].copy_(torch.from_numpy(np.ascontiguousarray(arr)))
         torch.cuda.current_stream(d["device"]).synchronize()
         obs = self._obs is not None
@@ -859,6 +1028,7 @@ class BatchedEnv(BatchedDoNothing):
         self.last_bus[:] = d["last_bus"].cpu().numpy(); self.line_cooldown[:] = d["line_cd"].cpu().numpy()
         self.sub_cooldown[:] = d["sub_cd"].cpu().numpy(); self.done[:] = d["done"].cpu().numpy()
         self.is_illegal = d["is_illegal"].cpu().numpy().copy(); self.current_step[:] = d["current_step"].cpu().numpy()
+        self.is_ambiguous = d["is_ambiguous"].cpu().numpy().copy()
         self._nb_inst[:] = s["nb_inst"]; self._cap_dirty[:] = s["cap_dirty"]
         if self._obs is not None:
             self._obs["reset"][:] = s["obs_reset"]
@@ -879,7 +1049,7 @@ class BatchedEnv(BatchedDoNothing):
             self.nb_cap = self._bus_cap()
 
     def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
-                     raise_alarm=None):
+                     raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None):
         """:meth:`step` with the actions as CUDA tensors and the state kept on the device: ``sub_id`` int32 / int64 [B] (-1: none)
         with ``sub_bus`` int8 / int32 / int64 [B, >= max_sub_size]; ``line_id`` int32 / int64 [B] (-1: none) with ``line_status``
         int32 / int64 [B] (> 0 reconnect / < 0 disconnect).  Same semantics and bit-identical state as :meth:`step`; ordered against torch's current
@@ -890,12 +1060,29 @@ class BatchedEnv(BatchedDoNothing):
         range raises ValueError and changes nothing.  ``raise_alert``: bool / uint8 CUDA tensor [B, dim_alerts] (:meth:`enable_alerts`;
         None: no alert); ``info["rewards"]["alert"]`` is then the environment's float64 [B] buffer of the AlertReward.
         ``raise_alarm``: bool / uint8 CUDA tensor [B, dim_alarms] (:meth:`enable_alarms`; None: no alarm); ``info["rewards"]["alarm"]``
-        and ``info["is_alarm_illegal"]`` are then the environment's float64 / bool [B] buffers."""
+        and ``info["is_alarm_illegal"]`` are then the environment's float64 / bool [B] buffers.
+        The vector action of :meth:`step` as CUDA tensors: ``set_bus`` int8 [B, dim_topo], ``change_bus`` bool [B, dim_topo],
+        ``set_line_status`` int8 [B, n_line], ``change_line_status`` bool [B, n_line] (any subset, not with sub_id / line_id), copied
+        on the device into the environment's buffers; ``info["is_ambiguous"]`` is then its bool [B] buffer.  A value out of range
+        raises ValueError from the validation launch and changes nothing."""
         import torch
         d = self._tensor_state()
         dev, B = d["device"], self.batch
         if (sub_id is None) != (sub_bus is None) or (line_id is None) != (line_status is None):
             raise ValueError("sub_id / sub_bus and line_id / line_status come in pairs")
+        gm = self.gm
+        vec = [(set_bus, "set_bus", (B, gm.dim_topo), torch.int8), (change_bus, "change_bus", (B, gm.dim_topo), torch.bool),
+               (set_line_status, "set_line_status", (B, gm.n_line), torch.int8),
+               (change_line_status, "change_line_status", (B, gm.n_line), torch.bool)]
+        use_vec = any(x is not None for x, _, _, _ in vec)
+        if use_vec:
+            if sub_id is not None or line_id is not None:
+                raise ValueError("the vector action (set_bus, change_bus, set_line_status, change_line_status) replaces sub_id / line_id")
+            for x, name, shape, dt in vec:
+                if x is not None:
+                    _check_tensor(x, name, shape, (dt,), dev)
+            if change_bus is not None and gm.n_busbar != 2:
+                raise ValueError("change_bus needs two busbars per substation")
         ints = (torch.int32, torch.int64)
         keep = []
 
@@ -941,11 +1128,21 @@ class BatchedEnv(BatchedDoNothing):
                 d["alarm_raise"].zero_()
             else:
                 d["alarm_raise"].copy_(raise_alarm != 0)
+        if use_vec:                                       # (device to device, on torch's stream like the alert buffers)
+            for (x, _, _, _), key in zip(vec, ("act_set_bus", "act_change_bus", "act_set_status", "act_change_status")):
+                if x is None:
+                    d[key].zero_()
+                else:
+                    d[key].copy_(x)
         cur, eng = self._streams()
         eng.wait_stream(cur)
         try:
-            self.engine.env_step(sid, sbus, stride, cols, lid, lst, from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter,
-                                 tol_mva=self.tol_mva, tight_cap=self.tight_cap, stamp=self.n_steps + 1)
+            if use_vec:
+                self.engine.env_step_act(from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter, tol_mva=self.tol_mva,
+                                         tight_cap=self.tight_cap, stamp=self.n_steps + 1)
+            else:
+                self.engine.env_step(sid, sbus, stride, cols, lid, lst, from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter,
+                                     tol_mva=self.tol_mva, tight_cap=self.tight_cap, stamp=self.n_steps + 1)
         except RuntimeError as e:
             if "(-1)" in str(e):                          # B200PF_E_ARG: an action out of range, nothing was written
                 raise ValueError(str(e)) from None
@@ -960,6 +1157,8 @@ class BatchedEnv(BatchedDoNothing):
             self.nb_cap = st["nb_cap"]
         info = {"status": d["status"], "iters": d["iters"], "newly_done": d["newly_done"], "is_illegal": d["is_illegal"],
                 "disc_lines": d["disc"] if self.protections else None}
+        if use_vec:
+            info["is_ambiguous"] = d["is_ambiguous"]
         if self._opp is not None:
             info["opponent_attack_line"] = d["opp_lines"] if self._opp.multi else d["opp_line"]
             info["opponent_attack_duration"] = d["opp_dur"]

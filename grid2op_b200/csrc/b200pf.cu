@@ -142,6 +142,9 @@ struct b200pf_handle {
     // alarms of the device environment (b200pf_alarm_bind)
     AlarmArgs alarm{}; int alarm_batch = 0;
     DevBufs alarm_bufs;
+    // the agent's action rules and vector-action buffers of the device environment (b200pf_act_bind)
+    ActArgs act{}; int act_batch = 0;
+    DevBufs act_bufs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -356,6 +359,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     h->opp_bufs.release();
     h->alert_bufs.release();
     h->alarm_bufs.release();
+    h->act_bufs.release();
     delete h;
     return 0;
 }
@@ -1960,7 +1964,7 @@ static inline unsigned env_grid(int n) { return (unsigned)((n + 127) / 128); }
 // the attacked lines the opponent of the same launches writes), the alarms (n = 0: none) and the observe input record (NULL when
 // the observation layer is not bound to this series).  An error when a GeometricOpponent lacks its schedules, a multi-area one its
 // areas, or when the observation layer's alert or alarm values do not match the bound alerts or alarms.
-struct EnvLayers { OppArgs opp; AlertArgs al; AlarmArgs am; int32_t *obs_rec; int obs_stride; };
+struct EnvLayers { OppArgs opp; AlertArgs al; AlarmArgs am; ActArgs act; int32_t *obs_rec; int obs_stride; };
 static int env_layers(const b200pf_handle *h, EnvLayers *l) {
     if (h->opp_batch && h->opp.kind == OPP_GEOMETRIC && !h->opp_geo_bound)
         return fail(B200PF_E_STATE, "GeometricOpponent bound without its schedules (b200pf_opp_geo_bind)");
@@ -1978,6 +1982,7 @@ static int env_layers(const b200pf_handle *h, EnvLayers *l) {
         else if (l->opp.kind != OPP_NONE) { l->al.attack = l->opp.attack_line; l->al.attack_stride = 1; }
     }
     l->am = layer_bound(h, h->alarm_batch) ? h->alarm : AlarmArgs{};
+    l->act = layer_bound(h, h->act_batch) ? h->act : ActArgs{};      // (aff_sub NULL: no rules bound, DefaultRules at 1 / 1)
     const bool obs = obs_bound(h);
     l->obs_rec = obs ? h->d_obs_in : nullptr;
     l->obs_stride = obs_stride(h);
@@ -1988,15 +1993,18 @@ static int env_layers(const b200pf_handle *h, EnvLayers *l) {
     return 0;
 }
 
-extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
-                               const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter,
-                               double tol_mva, int tight_cap, int stamp) {
+// b200pf_env_step and b200pf_env_step_act: vec = 1 takes the step's action from the vector buffers of b200pf_act_bind
+static int env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
+                    const int32_t *d_line_id, const int32_t *d_line_status, int vec, int from_reset, int is_dc, int max_iter,
+                    double tol_mva, int tight_cap, int stamp) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
+    if (vec && !layer_bound(h, h->act_batch)) return fail(B200PF_E_STATE, "no action buffers bound to the current environment (b200pf_act_bind)");
     EnvLayers l;
     TRY(env_layers(h, &l));
+    l.act.vec = vec && !from_reset ? 1 : 0;
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2008,18 +2016,21 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     a.from_reset = from_reset ? 1 : 0; a.tight_cap = tight_cap ? 1 : 0; a.prot = h->prot;
     // 1. validation + apply (the apply kernel writes nothing when an input was rejected)
     CU(cudaMemsetAsync(a.ctl, 0, ENV_CTL_WORDS * 4, h->stream));
-    if (a.sub_id || a.line_id) {
-        pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a);
+    if (a.sub_id || a.line_id || l.act.vec) {
+        pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a, l.act);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi);
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.act);
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     h->env_d2h += ENV_CTL_WORDS * 4; h->env_waits++;
     const int32_t *c = h->h_env_ctl;
-    if (c[ENV_CTL_ERR]) return fail(B200PF_E_ARG, "action out of range (substation / line id outside [-1, n), busbar outside [-1, n_busbar])");
+    if (c[ENV_CTL_ERR])
+        return fail(B200PF_E_ARG, l.act.vec ? "vector action out of range (busbar outside [-1, n_busbar], -1 on an element other than a line end, "
+                                              "change_bus without two busbars, line status outside {-1, 0, 1}, or a flag other than 0 / 1)"
+                                            : "action out of range (substation / line id outside [-1, n), busbar outside [-1, n_busbar])");
     h->env_illegal += c[ENV_CTL_N_ILLEGAL];
     int nb_cap = 0;
     if (tight_cap) {
@@ -2058,9 +2069,58 @@ extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const 
     a.status = h->x_status ? h->x_status : h->d_status;
     a.disc = h->prot ? h->d_disc : nullptr;
     a.obs_in = l.obs_rec; a.obs_stride = l.obs_stride; a.stamp = stamp;
-    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, l.al, l.am);
+    pf_kernel_env_post<<<env_grid(B), 128, 0, h->stream>>>(a, l.al, l.am, l.act);
     CU(cudaGetLastError());
     h->env_steps++;
+    return 0;
+}
+
+extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
+                               const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter,
+                               double tol_mva, int tight_cap, int stamp) {
+    return env_step(h, d_sub_id, d_sub_bus, sub_bus_stride, sub_bus_cols, d_line_id, d_line_status, 0, from_reset, is_dc, max_iter, tol_mva,
+                    tight_cap, stamp);
+}
+
+extern "C" int b200pf_env_step_act(b200pf_handle *h, int from_reset, int is_dc, int max_iter, double tol_mva, int tight_cap, int stamp) {
+    return env_step(h, nullptr, nullptr, 0, 0, nullptr, nullptr, 1, from_reset, is_dc, max_iter, tol_mva, tight_cap, stamp);
+}
+
+extern "C" int b200pf_act_bind(b200pf_handle *h, const b200pf_act_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
+    const HostGrid &hg = h->hg;
+    if (d->max_sub_changed < 0 || d->max_line_status_changed < 0 || d->n_area < 0 || d->n_area > ACT_MAX_AREA ||
+        (d->n_area && (!d->sub_area || !d->line_area)))
+        return fail(B200PF_E_ARG, "bad action rules");
+    if (!d->set_bus || !d->change_bus || !d->set_status || !d->change_status || !d->is_ambiguous) return fail(B200PF_E_ARG, "action buffers missing");
+    if (d->n_area) {
+        const uint32_t areas = d->n_area == 32 ? 0xffffffffu : (1u << d->n_area) - 1u;
+        for (int s = 0; s < hg.n_sub; ++s) if (d->sub_area[s] & ~areas) return fail(B200PF_E_ARG, "a substation in an area past n_area");
+        for (int l = 0; l < hg.n_line; ++l) if (d->line_area[l] & ~areas) return fail(B200PF_E_ARG, "a line in an area past n_area");
+    }
+    TRY(unbind(h, &h->act_batch, h->act_bufs));
+    // the substation of every topology position (the shunts sit past dim_topo)
+    std::vector<int32_t> sub_of_pos(hg.dim_topo, 0);
+    for (int k = 0; k < hg.n_line; ++k) { sub_of_pos[hg.line_or_pos[k]] = hg.line_or_sub[k]; sub_of_pos[hg.line_ex_pos[k]] = hg.line_ex_sub[k]; }
+    for (int k = 0; k < hg.n_unit; ++k) if (hg.unit_pos[k] >= 0 && hg.unit_pos[k] < hg.dim_topo) sub_of_pos[hg.unit_pos[k]] = hg.unit_sub[k];
+    for (int k = 0; k < hg.n_load; ++k) sub_of_pos[hg.load_pos[k]] = hg.load_sub[k];
+    for (int k = 0; k < hg.n_sto; ++k) sub_of_pos[hg.sto_pos[k]] = hg.sto_sub[k];
+    const size_t B = (size_t)h->env_batch;
+    ActArgs r{};
+    r.max_sub = d->max_sub_changed; r.max_line = d->max_line_status_changed; r.n_area = d->n_area;
+    DevBufs &o = h->act_bufs;
+    TRY(dev_alloc(h, o, r.sub_of_pos, sub_of_pos.size() * 4, sub_of_pos.data()));
+    if (d->n_area) {
+        TRY(dev_alloc(h, o, r.sub_area, (size_t)hg.n_sub * 4, d->sub_area));
+        TRY(dev_alloc(h, o, r.line_area, (size_t)hg.n_line * 4, d->line_area));
+    }
+    TRY(dev_alloc(h, o, r.aff_sub, B * (size_t)hg.n_sub, nullptr, 0));
+    r.set_bus = d->set_bus; r.change_bus = d->change_bus; r.set_status = d->set_status; r.change_status = d->change_status;
+    r.is_ambiguous = d->is_ambiguous;
+    CU(cudaMemsetAsync(r.is_ambiguous, 0, B, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    h->act = r; h->act_batch = (int)B;
     return 0;
 }
 
@@ -2076,7 +2136,7 @@ extern "C" int b200pf_env_reset(b200pf_handle *h, const uint8_t *d_mask, const i
     EnvArgs a = h->env;
     a.reset_mask = d_mask; a.reset_rows = d_rows;
     a.obs_in = l.obs_rec; a.obs_stride = l.obs_stride;
-    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.al, l.am);
+    pf_kernel_env_reset<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.al, l.am, l.act);
     CU(cudaGetLastError());
     // the plans of the reset rows, looked up now and over the same topology as b200pf_series_reset_instances does for the host
     // path, so that both paths make the same plan lookups in the same calls (which plans a call builds, their ids, and the kernel

@@ -3,8 +3,10 @@
 // isolated-busbar rule, cooldowns, game over, the observe layer's per-instance input record).
 //
 // Every body restates, per instance, the numpy code of grid2op_b200/batched_env.py in the same order:
-//   env_apply_instance   BatchedEnv._apply_agent, then _apply_environment (and the bus count of _bus_cap), with the opponent's
-//                        decision before the agent's action and its attack after the outages when one is bound (b200pf_opp.cuh);
+//   env_apply_instance   BatchedEnv._apply_agent (or, with the vector action, _apply_actions: act_vec_instance), then
+//                        _apply_environment (and the bus count of _bus_cap), with the opponent's decision before the agent's action
+//                        and its attack after the outages when one is bound (b200pf_opp.cuh); both encodings share the legality
+//                        rules of BatchedEnv._illegal (ActLegal);
 //   env_post_instance    the rest of BatchedEnv.step behind the solve;
 //   env_reset_instance   BatchedEnv.reset_instances (with the library's part, b200pf_series_reset_instances, and the opponent's).
 // With line alerts bound (b200pf_alert.cuh), the post body updates the alert state and the AlertReward after the step's attack,
@@ -76,6 +78,26 @@ struct EnvArgs {
     const uint8_t *reset_mask; const int32_t *reset_rows;
 };
 
+enum { ACT_MAX_AREA = 16 };            // RulesByArea areas the legality counts handle
+
+// The agent's action rules and grid2op's native topology action (b200pf_act_bind).  The rules apply to both encodings: LookParam
+// (MAX_SUB_CHANGED / MAX_LINE_STATUS_CHANGED over the whole grid; n_area = 0) or RulesByArea._lookparam_byarea (the same maxima per
+// area: a substation counts in the areas of its mask bits, a line in those of its origin substation), and PreventReconnection.
+// With vec = 1 the step's action is the four vectors below instead of EnvArgs' sub_id / line_id pair.
+struct ActArgs {
+    int max_sub, max_line;                          // MAX_SUB_CHANGED, MAX_LINE_STATUS_CHANGED
+    int n_area;                                     // 0: LookParam over the whole grid
+    const uint32_t *sub_area, *line_area;           // [n_sub], [n_line] area masks (n_area > 0)
+    const int32_t *sub_of_pos;                      // [dim_topo] substation of each topology position
+    int vec;                                        // this step's action is the vector action
+    const int8_t *set_bus;                          // [batch][dim_topo] 0 leave, -1 disconnect (line ends), 1..n_busbar
+    const uint8_t *change_bus;                      // [batch][dim_topo] 0 / 1 (two busbars per substation)
+    const int8_t *set_status;                       // [batch][n_line] -1 / 0 / +1
+    const uint8_t *change_status;                   // [batch][n_line] 0 / 1
+    uint8_t *is_ambiguous;                          // [batch] caller-owned: the action was replaced by "do nothing" as ambiguous
+    uint8_t *aff_sub;                               // [batch][n_sub] library scratch: substations the legal vector action touched
+};
+
 #if defined(__CUDA_ARCH__)
 #define ENV_ATOMIC_ADD(p, v) atomicAdd((p), (v))
 #define ENV_ATOMIC_MAX(p, v) atomicMax((p), (v))
@@ -104,6 +126,159 @@ ENV_HD inline bool env_input_ok(const EnvArgs &a, int i) {
     return true;
 }
 
+// The vector action of instance i: busbars in [-1, n_busbar] with -1 on line ends only (detaching a load, generator or storage unit
+// is not restated), change_bus only with two busbars per substation, line statuses in {-1, 0, 1}.
+ENV_HD inline bool act_input_ok(const EnvArgs &a, const ActArgs &r, int i) {
+    const int8_t *sb = r.set_bus + (size_t)i * a.dim_topo;
+    const uint8_t *cb = r.change_bus + (size_t)i * a.dim_topo;
+    for (int p = 0; p < a.dim_topo; ++p) {
+        if (sb[p] < -1 || sb[p] > a.n_busbar || (sb[p] == -1 && a.line_of_pos[p] < 0)) return false;
+        if (cb[p] > 1 || (cb[p] && a.n_busbar != 2)) return false;
+    }
+    const int8_t *ss = r.set_status + (size_t)i * a.n_line;
+    const uint8_t *cs = r.change_status + (size_t)i * a.n_line;
+    for (int l = 0; l < a.n_line; ++l)
+        if (ss[l] < -1 || ss[l] > 1 || cs[l] > 1) return false;
+    return true;
+}
+
+// What an action's topological impact counts for the legality rules: lines and substations per area (one area without
+// RulesByArea), and whether one of them is in cooldown (PreventReconnection).  Both encodings fill it, one element at a time.
+struct ActLegal {
+    int n_line[ACT_MAX_AREA], n_sub[ACT_MAX_AREA];
+    bool cooldown;
+};
+
+ENV_HD inline void act_legal_init(ActLegal &c) {
+    for (int k = 0; k < ACT_MAX_AREA; ++k) { c.n_line[k] = 0; c.n_sub[k] = 0; }
+    c.cooldown = false;
+}
+
+ENV_HD inline void act_count(const ActArgs *r, const uint32_t *area, int id, int *n) {
+    if (!r || !r->n_area) { n[0] += 1; return; }
+    const uint32_t m = area[id];
+    for (int k = 0; k < r->n_area; ++k) n[k] += (int)((m >> k) & 1u);
+}
+
+ENV_HD inline void act_impact_line(ActLegal &c, const EnvArgs &a, const ActArgs *r, int i, int l) {
+    c.cooldown |= a.line_cd[(size_t)i * a.n_line + l] > 0;
+    act_count(r, r ? r->line_area : nullptr, l, c.n_line);
+}
+
+ENV_HD inline void act_impact_sub(ActLegal &c, const EnvArgs &a, const ActArgs *r, int i, int s) {
+    c.cooldown |= a.sub_cd[(size_t)i * a.n_sub + s] > 0;
+    act_count(r, r ? r->sub_area : nullptr, s, c.n_sub);
+}
+
+// LookParam (or RulesByArea's counts) and PreventReconnection; without bound rules, DefaultRules with both maxima at 1
+ENV_HD inline bool act_illegal(const ActLegal &c, const ActArgs *r) {
+    const int max_line = r ? r->max_line : 1, max_sub = r ? r->max_sub : 1, na = r && r->n_area ? r->n_area : 1;
+    bool bad = c.cooldown;
+    for (int k = 0; k < na; ++k) bad |= c.n_line[k] > max_line || c.n_sub[k] > max_sub;
+    return bad;
+}
+
+// _BackendAction's topology stage for one position: change_bus (connected elements toggle 1 <-> 2), then set_bus
+ENV_HD inline int act_topo_value(int v, uint8_t change, int8_t set) {
+    if (change && v > 0) v = 3 - v;
+    return set != 0 ? set : v;
+}
+
+// grid2op's native topology action for instance i (BaseEnv.step, baseEnv.py:3706-3767): ambiguity, topological impact on the line
+// status the previous step left, legality, and _BackendAction.__iadd__'s application (line status change then set, change_bus then
+// set_bus, then the reconciliation of disconnected / reconnected line ends).  A disconnected end is one <= 0.  Writes is_ambiguous,
+// is_illegal, the impacted lines (affl) and substations (aff_sub) of a legal action; -> the topology may have changed.
+ENV_HD inline bool act_vec_instance(const EnvArgs &a, const ActArgs &r, int i, bool done, uint8_t *affl) {
+    const int nl = a.n_line, ns = a.n_sub, nt = a.dim_topo;
+    int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
+    int8_t *lb = a.last_bus + (size_t)i * nt;
+    const int8_t *sb = r.set_bus + (size_t)i * nt;
+    const uint8_t *cb = r.change_bus + (size_t)i * nt;
+    const int8_t *ss = r.set_status + (size_t)i * nl;
+    const uint8_t *cs = r.change_status + (size_t)i * nl;
+    uint8_t *affs = r.aff_sub + (size_t)i * ns;
+    for (int s = 0; s < ns; ++s) affs[s] = 0;
+    // 1. BaseAction._check_for_ambiguity, topology part (baseAction.py:3558-3565, :3670-3771)
+    bool any = false, amb = false;
+    for (int p = 0; p < nt; ++p) {
+        amb |= sb[p] != 0 && cb[p];
+        any |= sb[p] != 0 || cb[p];
+    }
+    for (int l = 0; l < nl; ++l) {
+        const int so = sb[a.line_or_pos[l]], se = sb[a.line_ex_pos[l]];
+        const bool ch = cb[a.line_or_pos[l]] || cb[a.line_ex_pos[l]];
+        amb |= ss[l] != 0 && cs[l];
+        amb |= (so == -1 && se > 0) || (se == -1 && so > 0);
+        amb |= ss[l] == -1 && (so > 0 || se > 0 || ch);
+        amb |= ss[l] == 1 && (so == -1 || se == -1 || ch);
+        any |= ss[l] != 0 || cs[l];
+    }
+    amb = amb && !done;
+    r.is_ambiguous[i] = amb ? 1 : 0;
+    // 2. get_topological_impact (baseAction.py:1796-2022): the lines whose status the action sets, changes, or reaches through a
+    // busbar of one end; the substations of the remaining bus changes (ends of those lines excluded when they reconnect a line or
+    // the status action targets a disconnected line)
+    ActLegal c;
+    act_legal_init(c);
+    for (int l = 0; l < nl; ++l) {
+        const int po = a.line_or_pos[l], pe = a.line_ex_pos[l];
+        const bool on = tv[po] > 0 && tv[pe] > 0, named = cs[l] || ss[l] != 0;
+        const bool conn = (sb[po] > 0 || sb[pe] > 0) && !on, disc = (sb[po] < 0 || sb[pe] < 0) && on;
+        affl[l] = (named || conn || disc) ? 1 : 0;
+        if (affl[l]) act_impact_line(c, a, &r, i, l);
+    }
+    for (int p = 0; p < nt; ++p) {
+        if (!(cb[p] || sb[p] != 0)) continue;
+        const int l = a.line_of_pos[p];
+        if (l >= 0) {                                         // an end of an impacted line that was out, or of one it disconnects
+            const int po = a.line_or_pos[l], pe = a.line_ex_pos[l];
+            const bool on = tv[po] > 0 && tv[pe] > 0;
+            if (on ? (sb[po] < 0 || sb[pe] < 0) : affl[l] != 0) continue;
+        }
+        const int s = r.sub_of_pos[p];
+        if (!affs[s]) { affs[s] = 1; act_impact_sub(c, a, &r, i, s); }
+    }
+    // 3. legality; an ambiguous, illegal or finished instance's action is "do nothing"
+    const bool illegal = !amb && act_illegal(c, &r);
+    const bool counted = illegal && !done;
+    a.is_illegal[i] = counted ? 1 : 0;
+    if (counted) ENV_ATOMIC_ADD(&a.ctl[ENV_CTL_N_ILLEGAL], 1);
+    if (amb || illegal || done) {
+        for (int l = 0; l < nl; ++l) affl[l] = 0;
+        for (int s = 0; s < ns; ++s) affs[s] = 0;
+        return false;
+    }
+    if (!any) return false;
+    // 4. _BackendAction.__iadd__ (_backendAction.py:738-765, :810-919), with the busbars last registered (last_bus)
+    for (int l = 0; l < nl; ++l) {
+        const int po = a.line_or_pos[l], pe = a.line_ex_pos[l];
+        int vo = tv[po], ve = tv[pe];
+        if (cs[l]) {                                          // change_status
+            if (vo > 0 || ve > 0) { vo = -1; ve = -1; }
+            else { vo = lb[po]; ve = lb[pe]; }
+        }
+        if (ss[l] < 0) { vo = -1; ve = -1; }                  // set_status
+        else if (ss[l] > 0) {
+            if (vo <= 0) vo = lb[po];
+            if (ve <= 0) ve = lb[pe];
+        }
+        const bool before_off = vo <= 0;                      // _status_or_before
+        const bool disco = before_off || ve <= 0;
+        vo = act_topo_value(vo, cb[po], sb[po]);
+        ve = act_topo_value(ve, cb[pe], sb[pe]);
+        if (before_off && (vo > 0 || ve > 0)) {               // _aux_iadd_reconcile_disco_reco: reconnected, the other end on its last busbar
+            if (vo <= 0) vo = lb[po];
+            if (ve <= 0) ve = lb[pe];
+        } else if (disco || vo <= 0 || ve <= 0) { vo = -1; ve = -1; }
+        tv[po] = (int8_t)vo; tv[pe] = (int8_t)ve;
+    }
+    for (int p = 0; p < nt; ++p)
+        if (a.line_of_pos[p] < 0) tv[p] = (int8_t)act_topo_value(tv[p], cb[p], sb[p]);
+    for (int p = 0; p < nt; ++p)                              // last_topo_registered.update_connected
+        if (tv[p] > 0) lb[p] = tv[p];
+    return true;
+}
+
 // active buses of one topology record (b200pf_grid_max_active_buses)
 ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
     uint32_t bits[ENV_MAX_SLOT / 32];
@@ -127,15 +302,15 @@ ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
     return n;
 }
 
-// BatchedEnv._apply_agent followed by _apply_environment and the opponent's attack (o: NULL or no opponent bound), for instance i
-// (g: the GeometricOpponent's part, m: the GeometricOpponentMultiArea's; NULL for the other kinds)
+// BatchedEnv._apply_agent (or _apply_actions, ac->vec) followed by _apply_environment and the opponent's attack (o: NULL or no
+// opponent bound), for instance i (g: the GeometricOpponent's part, m: the GeometricOpponentMultiArea's; NULL for the other kinds;
+// ac: NULL or the bound action rules)
 ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
-                                      const OppMultiArgs *m = nullptr) {
+                                      const OppMultiArgs *m = nullptr, const ActArgs *ac = nullptr) {
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * a.dim_topo;
     uint8_t *affl = a.aff_l + (size_t)i * nl;
-    const int32_t *lcd = a.line_cd + (size_t)i * nl;
     for (int l = 0; l < nl; ++l) affl[l] = 0;
     a.aff_s[i] = -1;
     const bool done = a.done[i] != 0;
@@ -147,7 +322,10 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
         else if (m) opp_multi_none(*m, i);
         o->attack_line[i] = opp_line; o->attack_dur[i] = opp_dur;
     }
-    if (!a.from_reset) {
+    if (ac && ac->is_ambiguous && (a.from_reset || !ac->vec)) ac->is_ambiguous[i] = 0;
+    if (!a.from_reset && ac && ac->vec) {
+        dirty = act_vec_instance(a, *ac, i, done, affl);
+    } else if (!a.from_reset) {
         bool has_sub = false, has_line = false;
         int sid = -1, lid = -1, lst = 0;
         const int8_t *bus = nullptr;
@@ -163,8 +341,11 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
             has_line = lid >= 0 && lst != 0;
         }
         // a busbar > 0 for the end of a disconnected line reconnects that line (baseAction.py:1836-1860)
+        // (each reconnecting entry counts as one line, as BatchedEnv._apply_agent counts them)
+        ActLegal c;
+        act_legal_init(c);
         int n_reco = 0;
-        bool reco_in_cd = false, reco_is_line = false, m_not_reco = false, sub_impacted = has_sub;
+        bool reco_is_line = false, m_not_reco = false, sub_impacted = has_sub;
         const int32_t *pos = has_sub ? a.sub_pos + (size_t)sid * a.max_sub : nullptr;
         if (has_sub) {
             for (int k = 0; k < a.max_sub; ++k) {
@@ -173,22 +354,16 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
                 const int lp = a.line_of_pos[p];
                 if (tv[p] <= 0 && lp >= 0) {
                     ++n_reco;
-                    reco_in_cd |= lcd[lp] > 0;
+                    act_impact_line(c, a, ac, i, lp);
                     reco_is_line |= has_line && lp == lid;
                 } else m_not_reco = true;
             }
             if (n_reco) sub_impacted = m_not_reco;
+            if (sub_impacted) act_impact_sub(c, a, ac, i, sid);
         }
-        // DefaultRules legality; finished instances ignore their action
-        bool illegal = false;
-        if (has_sub) {
-            illegal |= sub_impacted && a.sub_cd[(size_t)i * a.n_sub + sid] > 0;
-            if (n_reco) {
-                illegal |= reco_in_cd;
-                illegal |= n_reco + (has_line && !reco_is_line ? 1 : 0) > 1;
-            }
-        }
-        if (has_line) illegal |= lcd[lid] > 0;
+        if (has_line && !reco_is_line) act_impact_line(c, a, ac, i, lid);
+        // the legality rules; finished instances ignore their action
+        const bool illegal = act_illegal(c, ac);
         const bool counted = illegal && !done;
         a.is_illegal[i] = counted ? 1 : 0;
         if (counted) ENV_ATOMIC_ADD(&a.ctl[ENV_CTL_N_ILLEGAL], 1);
@@ -265,8 +440,10 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     }
 }
 
-// the rest of BatchedEnv.step behind the solve, for instance i (al: NULL or the line alerts, am: NULL or the alarms)
-ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr) {
+// the rest of BatchedEnv.step behind the solve, for instance i (al: NULL or the line alerts, am: NULL or the alarms, ac: NULL or the
+// bound action rules)
+ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr,
+                                     const ActArgs *ac = nullptr) {
     const int nl = a.n_line, ns = a.n_sub;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     const bool live = a.done[i] == 0;
@@ -315,7 +492,12 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
         for (int s = 0; s < ns; ++s)
             if (sc[s] > 0 && live) sc[s] -= 1;
         if (a.aff_s[i] >= 0) sc[a.aff_s[i]] = a.cd_sub;
+        if (ac && ac->vec)
+            for (int s = 0; s < ns; ++s)
+                if (ac->aff_sub[(size_t)i * ns + s]) sc[s] = a.cd_sub;
     }
+    // an ambiguous action was "do nothing": not illegal, but rewarded as one and registering no alarm
+    const bool ambiguous = ac && ac->is_ambiguous && ac->is_ambiguous[i];
     const bool newly = live && st != 0;
     a.newly_done[i] = newly ? 1 : 0;
     if (newly) a.done[i] = 1;
@@ -334,7 +516,7 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
     const bool alarms = am && am->n;
     if (alarms) {                                             // an instance finished before the step keeps its alarm state
         if (live && !a.from_reset) {
-            alarm_register_instance(*am, i, a.current_step[i], a.is_illegal[i] != 0);
+            alarm_register_instance(*am, i, a.current_step[i], a.is_illegal[i] != 0 || ambiguous);
             if (am->reward && newly) alarm_reward_instance(*am, i, a.current_step[i], disc);
             else am->reward_out[i] = 0.0;
         } else { am->illegal[i] = 0; am->reward_out[i] = 0.0; }
@@ -344,7 +526,7 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
         for (int l = 0; l < nl; ++l) h[l] = lc[l];
         for (int s = 0; s < ns; ++s) h[nl + s] = sc[s];
         h[nl + ns] = a.current_step[i]; h[nl + ns + 1] = a.stamp;
-        h[nl + ns + 2] = (a.is_illegal[i] ? 1 : 0) + (a.done[i] ? 2 : 0) + (a.obs_reset[i] ? 4 : 0);
+        h[nl + ns + 2] = (a.is_illegal[i] ? 1 : 0) + (a.done[i] ? 2 : 0) + (a.obs_reset[i] ? 4 : 0) + (ambiguous ? 8 : 0);
         if (alerts) alert_obs_record(*al, i, h + nl + ns + 3);
         if (alarms) alarm_obs_record(*am, i, a.current_step[i], h + nl + ns + 3 + (alerts ? 6 * al->n + 1 : 0));
     }
@@ -352,8 +534,10 @@ ENV_HD inline void env_post_instance(const EnvArgs &a, int i, const AlertArgs *a
 
 // BatchedEnv.reset_instances for the instances of the mask (rows: next chronics row, default t0), opponent state included
 ENV_HD inline void env_reset_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
-                                      const OppMultiArgs *m = nullptr, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr) {
+                                      const OppMultiArgs *m = nullptr, const AlertArgs *al = nullptr, const AlarmArgs *am = nullptr,
+                                      const ActArgs *ac = nullptr) {
     if (!a.reset_mask[i]) return;
+    if (ac && ac->is_ambiguous) ac->is_ambiguous[i] = 0;
     if (al && al->n) alert_reset_instance(*al, i);
     if (am && am->n) alarm_reset_instance(*am, i);
     if (o && o->kind != OPP_NONE) opp_reset_instance(*o, i);
@@ -397,28 +581,31 @@ ENV_HD inline void env_observed_instance(const EnvArgs &a, int i) {
 }
 
 #if defined(__CUDACC__)
-__global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a) {
+// (r.aff_sub is NULL when no action rules are bound)
+__global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a, ActArgs r) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch && !env_input_ok(a, i)) atomicOr(&a.ctl[ENV_CTL_ERR], 1);
+    if (i < a.batch && !(r.vec ? act_input_ok(a, r, i) : env_input_ok(a, i))) atomicOr(&a.ctl[ENV_CTL_ERR], 1);
 }
 
 // one thread per instance; nothing is written when the validation flagged an input
-__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m) {
+__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, ActArgs r) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.batch || *(volatile int32_t *)&a.ctl[ENV_CTL_ERR]) return;
-    env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr);
+    env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr,
+                       r.aff_sub ? &r : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al, AlarmArgs am) {
+__global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al, AlarmArgs am, ActArgs r) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch) env_post_instance(a, i, al.n ? &al : nullptr, am.n ? &am : nullptr);
+    if (i < a.batch) env_post_instance(a, i, al.n ? &al : nullptr, am.n ? &am : nullptr, r.aff_sub ? &r : nullptr);
 }
 
-__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, AlertArgs al, AlarmArgs am) {
+__global__ void __launch_bounds__(128) pf_kernel_env_reset(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, AlertArgs al, AlarmArgs am,
+                                                           ActArgs r) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < a.batch)
         env_reset_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr, al.n ? &al : nullptr,
-                           am.n ? &am : nullptr);
+                           am.n ? &am : nullptr, r.aff_sub ? &r : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_observed(EnvArgs a) {

@@ -48,7 +48,7 @@ enum ObsSrc : int32_t {
 enum { OBS_REWARD_NONE = 0, OBS_REWARD_REDISP = 1, OBS_REWARD_L2RPN = 2 };
 
 // per-instance host input word flags (last int32 of the instance's host record)
-enum { OBS_F_ILLEGAL = 1, OBS_F_DONE = 2, OBS_F_RESET_COUNTERS = 4 };
+enum { OBS_F_ILLEGAL = 1, OBS_F_DONE = 2, OBS_F_RESET_COUNTERS = 4, OBS_F_AMBIGUOUS = 8 };
 
 struct ObsArgs {
     int batch;
@@ -258,7 +258,7 @@ OBS_HD inline float obs_reward(const ObsArgs &a, int inst, const double part[4])
     const int flags = hin[a.n_line + a.n_sub + 2];
     if (a.reward_kind == OBS_REWARD_L2RPN) return (flags & OBS_F_DONE) ? 0.f : (float)part[2];
     if (flags & OBS_F_DONE) return (float)a.reward_min;                  // game over = has_error
-    if (flags & OBS_F_ILLEGAL) return (float)a.reward_illegal;
+    if (flags & (OBS_F_ILLEGAL | OBS_F_AMBIGUOUS)) return (float)a.reward_illegal;   // reward_illegal_ambiguous
     const double mc = part[3] > -1e299 ? part[3] : 0.0;
     const double regret = (part[0] - part[1]) * a.dts_hours * mc;       // losses (MWh) x marginal cost; no redispatch, no storage
     return (float)((a.max_regret - regret) / part[1]);

@@ -46,7 +46,7 @@ ABI_SYMBOLS = (
     "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
     "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state",
     "b200pf_alert_bind", "b200pf_alert_get_state", "b200pf_alert_set_state",
-    "b200pf_alarm_bind", "b200pf_alarm_get_state", "b200pf_alarm_set_state",
+    "b200pf_alarm_bind", "b200pf_alarm_get_state", "b200pf_alarm_set_state", "b200pf_act_bind", "b200pf_env_step_act",
 )
 
 
@@ -132,6 +132,15 @@ class AlarmDesc(C.Structure):
         ("n_zone", C.c_int32), ("zone_mask", C.c_void_p), ("max_budget", C.c_float), ("budget_per_ts", C.c_float),
         ("alarm_cost", C.c_float), ("init_budget", C.c_float), ("best_time", C.c_int32), ("window_size", C.c_int32),
         ("reward", C.c_int32), ("raise_alarm", C.c_void_p), ("reward_out", C.c_void_p), ("is_alarm_illegal", C.c_void_p),
+    ]
+
+
+class ActDesc(C.Structure):
+    """``b200pf_act_desc`` of include/b200pf.h"""
+    _fields_ = [
+        ("max_sub_changed", C.c_int32), ("max_line_status_changed", C.c_int32), ("n_area", C.c_int32), ("sub_area", C.c_void_p),
+        ("line_area", C.c_void_p), ("set_bus", C.c_void_p), ("change_bus", C.c_void_p), ("set_status", C.c_void_p),
+        ("change_status", C.c_void_p), ("is_ambiguous", C.c_void_p),
     ]
 
 
@@ -318,12 +327,14 @@ def load_library():
     lib.b200pf_alarm_bind.argtypes = [vp, C.POINTER(AlarmDesc)]
     lib.b200pf_alarm_get_state.argtypes = [vp] + [vp] * 10
     lib.b200pf_alarm_set_state.argtypes = [vp] + [vp] * 10
+    lib.b200pf_act_bind.argtypes = [vp, C.POINTER(ActDesc)]
+    lib.b200pf_env_step_act.argtypes = [vp, i32, i32, i32, f64, i32, i32]
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
                "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
                "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state", "b200pf_alert_bind",
                "b200pf_alert_get_state", "b200pf_alert_set_state", "b200pf_alarm_bind", "b200pf_alarm_get_state",
-               "b200pf_alarm_set_state"):
+               "b200pf_alarm_set_state", "b200pf_act_bind", "b200pf_env_step_act"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -757,6 +768,27 @@ class PowerFlowEngine:
         self._check(self.lib.b200pf_env_step(self.h, v(sub_id), v(sub_bus), int(sub_bus_stride), int(sub_bus_cols), v(line_id),
                                              v(line_status), int(bool(from_reset)), int(bool(is_dc)), int(max_iter), float(tol_mva),
                                              int(bool(tight_cap)), int(stamp)), "b200pf_env_step")
+
+    def env_step_act(self, from_reset: bool = False, is_dc: bool = False, max_iter: int = 10, tol_mva: float = 1e-8, tight_cap: bool = True,
+                     stamp: int = 0):
+        """:meth:`env_step` with the action taken from the vector buffers :meth:`act_bind` bound (``b200pf_env_step_act``)"""
+        self._check(self.lib.b200pf_env_step_act(self.h, int(bool(from_reset)), int(bool(is_dc)), int(max_iter), float(tol_mva),
+                                                 int(bool(tight_cap)), int(stamp)), "b200pf_env_step_act")
+
+    def act_bind(self, max_sub_changed: int, max_line_status_changed: int, n_area: int, sub_area, line_area, d_set_bus: int,
+                 d_change_bus: int, d_set_status: int, d_change_status: int, d_is_ambiguous: int):
+        """the agent's action rules and the vector-action buffers of the device environment (``b200pf_act_bind``): ``n_area``
+        RulesByArea areas (0: none) with ``sub_area`` / ``line_area`` their uint32 masks [n_sub] / [n_line]; caller-owned device
+        buffers int8 / uint8 [B, dim_topo] (set_bus / change_bus), int8 / uint8 [B, n_line] (set / change line status) and uint8
+        [B] (is_ambiguous)"""
+        sa = la = None
+        if n_area:
+            sa, la = np.ascontiguousarray(sub_area, np.uint32), np.ascontiguousarray(line_area, np.uint32)
+        d = ActDesc(max_sub_changed=int(max_sub_changed), max_line_status_changed=int(max_line_status_changed), n_area=int(n_area),
+                    sub_area=None if sa is None else sa.ctypes.data, line_area=None if la is None else la.ctypes.data,
+                    set_bus=int(d_set_bus), change_bus=int(d_change_bus), set_status=int(d_set_status), change_status=int(d_change_status),
+                    is_ambiguous=int(d_is_ambiguous))
+        self._check(self.lib.b200pf_act_bind(self.h, C.byref(d)), "b200pf_act_bind")
 
     def env_reset(self, d_mask: int, d_rows: int = 0):
         self._check(self.lib.b200pf_env_reset(self.h, C.c_void_p(int(d_mask)), C.c_void_p(int(d_rows) or None)), "b200pf_env_reset")

@@ -395,6 +395,38 @@ int b200pf_env_pointers(b200pf_handle *h, int8_t **d_topo, int32_t **d_t, int32_
 int b200pf_observe_device(b200pf_handle *h, float *d_obs, float *d_reward);
 int b200pf_env_stats(const b200pf_handle *h, int64_t *out8);
 
+/* The agent's action rules and grid2op's native topology action for the device environment (csrc/b200pf_env.cuh, ActArgs).
+ * b200pf_act_bind needs a bound environment (b200pf_env_bind).  It copies the rules (host tables) and keeps the action buffers:
+ * caller-owned DEVICE buffers the caller writes before each b200pf_env_step_act, like the alerts' raise buffer.  Once bound, the rules
+ * apply to b200pf_env_step too: LookParam with max_sub_changed / max_line_status_changed over the whole grid (n_area = 0), or
+ * RulesByArea's per-area counts (sub_area / line_area: bit k set for a substation / line of area k, a line in the area of its
+ * origin substation; at most 16 areas), and PreventReconnection.  Without a bind, DefaultRules with both maxima at 1.
+ * b200pf_env_step_act is b200pf_env_step with the step's action taken from these buffers: set_bus int8 [batch][dim_topo] (0 leave,
+ * -1 disconnect a line end, 1..n_busbar), change_bus uint8 [batch][dim_topo] (0 / 1, two busbars per substation only), set_status
+ * int8 [batch][n_line] (-1 / 0 / +1), change_status uint8 [batch][n_line] (0 / 1).  Per live instance, in BaseEnv.step's order:
+ * BaseAction's topology ambiguity (an ambiguous action becomes "do nothing", is_ambiguous[i] = 1, is_illegal[i] = 0), the
+ * topological impact on the line status the previous step left, the rules above, and _BackendAction's application (line status
+ * change, then set, change_bus, then set_bus, then the reconnection / disconnection of line ends, last registered busbars from
+ * last_bus).  Every impacted line and substation gets its cooldown.  An entry out of range fails the call with B200PF_E_ARG before
+ * anything is written.  is_ambiguous uint8 [batch]: written by every step (0 on b200pf_env_step) and cleared by b200pf_env_reset;
+ * the observe record's flags word then carries B200PF_OBS_AMBIGUOUS (RedispReward pays reward_illegal for it), and an ambiguous
+ * action registers no alarm.  Host waits and bytes moved per step are those of b200pf_env_step. */
+enum { B200PF_OBS_AMBIGUOUS = 8 };
+typedef struct b200pf_act_desc {
+    int32_t max_sub_changed, max_line_status_changed;   /* MAX_SUB_CHANGED, MAX_LINE_STATUS_CHANGED */
+    int32_t n_area;                     /* RulesByArea areas, 0: none */
+    const uint32_t *sub_area;           /* [n_sub] area mask of each substation (n_area > 0) */
+    const uint32_t *line_area;          /* [n_line] area mask of each line (n_area > 0) */
+    /* caller-owned device buffers */
+    const int8_t *set_bus;              /* [batch][dim_topo] */
+    const uint8_t *change_bus;          /* [batch][dim_topo] */
+    const int8_t *set_status;           /* [batch][n_line] */
+    const uint8_t *change_status;       /* [batch][n_line] */
+    uint8_t *is_ambiguous;              /* [batch] */
+} b200pf_act_desc;
+int b200pf_act_bind(b200pf_handle *h, const b200pf_act_desc *desc);
+int b200pf_env_step_act(b200pf_handle *h, int from_reset, int is_dc, int max_iter, double tol_mva, int tight_cap, int stamp);
+
 /* Line-attack opponent of the device environment (csrc/b200pf_opp.cuh): grid2op's OpponentSpace with BaseActionBudget and a
  * RandomLineOpponent (kind 1) or a WeightedRandomOpponent (kind 2), attacking one line at a time with set_line_status -1, each
  * instance with its own numpy-legacy random stream (RandomState: MT19937 state of 624 words and a position, as get_state() gives
