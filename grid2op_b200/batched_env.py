@@ -128,6 +128,7 @@ class BatchedEnv(BatchedDoNothing):
         self._opp = None                                                   # line-attack opponent (:meth:`enable_opponent`)
         self._alerts = None                                                # line alerts (:meth:`enable_alerts`)
         self._alarms = None                                                # alarms (:meth:`enable_alarms`)
+        self._table = None                                                 # discrete action table (:meth:`set_action_table`)
 
     # ------------------------------------------------------------------------------------------------------------
     def _set_rules_by_area(self, areas):
@@ -378,6 +379,29 @@ class BatchedEnv(BatchedDoNothing):
             raise ValueError("set_line_status outside {-1, 0, 1}")
         return sb.astype(np.int8), cb, ss.astype(np.int8), cs
 
+    def set_action_table(self, table):
+        """Bind a discrete action table (:class:`grid2op_b200.action_table.ActionTable`, checked when it was built): ``step`` /
+        ``step_tensors(action_id=...)`` then act with row ``action_id[i]`` in instance i.  On the tensor path the library copies the
+        table to the device once.  A new call replaces the table; one built for another grid raises ValueError."""
+        if not table.matches(self.gm):
+            raise ValueError(f"action table for another grid (dim_topo {table.dim_topo}, n_line {table.n_line}, {table.n_busbar} busbars)")
+        if self._dev is not None:
+            self.engine.act_table_bind(table.set_bus, table.change_bus, table.set_line_status, table.change_line_status)
+        self._table = table
+
+    def _table_rows(self, action_id):
+        """``action_id`` int [B] checked against the bound table -> its rows (set_bus, change_bus, set_line_status,
+        change_line_status)"""
+        if self._table is None:
+            raise ValueError("action_id without an action table (set_action_table)")
+        a = np.asarray(action_id)
+        if a.shape != (self.batch,) or a.dtype.kind not in "iu":
+            raise ValueError(f"action_id must be an int array of shape {(self.batch,)}")
+        if ((a < 0) | (a >= self._table.n)).any():
+            raise ValueError(f"action_id outside [0, {self._table.n})")
+        t = self._table
+        return t.set_bus[a], t.change_bus[a], t.set_line_status[a], t.change_line_status[a]
+
     def _isolated_shunt_busbar(self) -> np.ndarray:
         """bool [B]: busbar 1 of a substation whose shunt is out of service in the grid file carries no element any more — for the
         reference an in-service bus without a voltage: ``runpf`` fails with "Isolated bus" (pandaPowerBackend.py:1241-1244) and the
@@ -415,7 +439,7 @@ class BatchedEnv(BatchedDoNothing):
                 self._cap_dirty[ii[was_on]] = True
 
     def step(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
-             raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None):
+             raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None, action_id=None):
         """One env.step of every instance.  ``sub_id`` int [B] (-1: none) with ``sub_bus`` int8 [B, >= max_sub_size] (busbar per
         element of that substation in topology-vector order, 0 = leave); ``line_id`` int [B] (-1: none) with ``line_status``
         int [B] (+1 reconnect / -1 disconnect); ``raise_alert`` bool [B, dim_alerts] (:meth:`enable_alerts`; None: no alert,
@@ -427,10 +451,18 @@ class BatchedEnv(BatchedDoNothing):
         ``change_bus`` bool [B, dim_topo] (two busbars per substation only), ``set_line_status`` int8 [B, n_line] in {-1, 0, 1},
         ``change_line_status`` bool [B, n_line]; :meth:`_apply_actions` restates what grid2op does with them.  ``info["is_ambiguous"]``
         (bool [B]) then says which actions were replaced by "do nothing" as ambiguous.  A value out of range, ``set_bus = -1`` on a
-        load, generator or storage unit, a wrong shape or dtype raise ValueError and change nothing."""
+        load, generator or storage unit, a wrong shape or dtype raise ValueError and change nothing.
+
+        ``action_id`` int [B] instead of any of the above: instance i acts with row ``action_id[i]`` of the table
+        :meth:`set_action_table` bound, as the vector action above (``info["is_ambiguous"]`` included).  An id outside [0, n),
+        no bound table, a wrong shape or dtype raise ValueError and change nothing."""
         vec = self._vector_action(set_bus, change_bus, set_line_status, change_line_status)
         if vec is not None and (sub_id is not None or line_id is not None):
             raise ValueError("the vector action (set_bus, change_bus, set_line_status, change_line_status) replaces sub_id / line_id")
+        if action_id is not None:
+            if vec is not None or sub_id is not None or line_id is not None:
+                raise ValueError("action_id replaces sub_id / line_id and the vector action")
+            vec = self._table_rows(action_id)
         if raise_alert is not None:
             if self._alerts is None:
                 raise ValueError("raise_alert without enable_alerts()")
@@ -937,6 +969,9 @@ class BatchedEnv(BatchedDoNothing):
         st["device"] = dev
         self._dev = st
         self._illegal_seen = 0
+        if self._table is not None:
+            t = self._table
+            self.engine.act_table_bind(t.set_bus, t.change_bus, t.set_line_status, t.change_line_status)
         if self._opp is not None:
             self._opp_bind_device()
         if self._alerts is not None:
@@ -1049,7 +1084,7 @@ class BatchedEnv(BatchedDoNothing):
             self.nb_cap = self._bus_cap()
 
     def step_tensors(self, sub_id=None, sub_bus=None, line_id=None, line_status=None, from_reset: bool = False, raise_alert=None,
-                     raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None):
+                     raise_alarm=None, set_bus=None, change_bus=None, set_line_status=None, change_line_status=None, action_id=None):
         """:meth:`step` with the actions as CUDA tensors and the state kept on the device: ``sub_id`` int32 / int64 [B] (-1: none)
         with ``sub_bus`` int8 / int32 / int64 [B, >= max_sub_size]; ``line_id`` int32 / int64 [B] (-1: none) with ``line_status``
         int32 / int64 [B] (> 0 reconnect / < 0 disconnect).  Same semantics and bit-identical state as :meth:`step`; ordered against torch's current
@@ -1064,7 +1099,10 @@ class BatchedEnv(BatchedDoNothing):
         The vector action of :meth:`step` as CUDA tensors: ``set_bus`` int8 [B, dim_topo], ``change_bus`` bool [B, dim_topo],
         ``set_line_status`` int8 [B, n_line], ``change_line_status`` bool [B, n_line] (any subset, not with sub_id / line_id), copied
         on the device into the environment's buffers; ``info["is_ambiguous"]`` is then its bool [B] buffer.  A value out of range
-        raises ValueError from the validation launch and changes nothing."""
+        raises ValueError from the validation launch and changes nothing.
+        ``action_id``: int32 / int64 CUDA tensor [B] instead of any of the above, ids into the table :meth:`set_action_table` bound
+        (copied to the device once, at the bind); each instance reads its own row inside the step's launches.  An id outside
+        [0, n) raises ValueError from the validation launch and changes nothing."""
         import torch
         d = self._tensor_state()
         dev, B = d["device"], self.batch
@@ -1083,6 +1121,11 @@ class BatchedEnv(BatchedDoNothing):
                     _check_tensor(x, name, shape, (dt,), dev)
             if change_bus is not None and gm.n_busbar != 2:
                 raise ValueError("change_bus needs two busbars per substation")
+        if action_id is not None:
+            if use_vec or sub_id is not None or line_id is not None:
+                raise ValueError("action_id replaces sub_id / line_id and the vector action")
+            if self._table is None:
+                raise ValueError("action_id without an action table (set_action_table)")
         ints = (torch.int32, torch.int64)
         keep = []
 
@@ -1108,6 +1151,7 @@ class BatchedEnv(BatchedDoNothing):
         if line_id is not None:
             lid = ids(line_id, "line_id")
             lst = ids(line_status, "line_status")
+        aid = ids(action_id, "action_id") if action_id is not None else 0
         if raise_alert is not None:
             if self._alerts is None:
                 raise ValueError("raise_alert without enable_alerts()")
@@ -1137,7 +1181,10 @@ class BatchedEnv(BatchedDoNothing):
         cur, eng = self._streams()
         eng.wait_stream(cur)
         try:
-            if use_vec:
+            if aid:
+                self.engine.env_step_ids(aid, from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter, tol_mva=self.tol_mva,
+                                         tight_cap=self.tight_cap, stamp=self.n_steps + 1)
+            elif use_vec:
                 self.engine.env_step_act(from_reset=from_reset, is_dc=self.is_dc, max_iter=self.max_iter, tol_mva=self.tol_mva,
                                          tight_cap=self.tight_cap, stamp=self.n_steps + 1)
             else:
@@ -1157,7 +1204,7 @@ class BatchedEnv(BatchedDoNothing):
             self.nb_cap = st["nb_cap"]
         info = {"status": d["status"], "iters": d["iters"], "newly_done": d["newly_done"], "is_illegal": d["is_illegal"],
                 "disc_lines": d["disc"] if self.protections else None}
-        if use_vec:
+        if use_vec or aid:
             info["is_ambiguous"] = d["is_ambiguous"]
         if self._opp is not None:
             info["opponent_attack_line"] = d["opp_lines"] if self._opp.multi else d["opp_line"]

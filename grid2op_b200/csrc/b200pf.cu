@@ -145,6 +145,10 @@ struct b200pf_handle {
     // the agent's action rules and vector-action buffers of the device environment (b200pf_act_bind)
     ActArgs act{}; int act_batch = 0;
     DevBufs act_bufs;
+    // the discrete action table of the device environment (b200pf_act_table_bind): n_act rows in the layout of the vector buffers
+    int n_act = 0;
+    int8_t *tab_set_bus = nullptr, *tab_set_status = nullptr; uint8_t *tab_change_bus = nullptr, *tab_change_status = nullptr;
+    DevBufs act_table_bufs;
 };
 
 // Host -> device copy of caller memory (pageable as a rule) that launches on ANY stream of the handle may read afterwards.  A plain
@@ -360,6 +364,7 @@ extern "C" int b200pf_destroy(b200pf_handle *h) {
     h->alert_bufs.release();
     h->alarm_bufs.release();
     h->act_bufs.release();
+    h->act_table_bufs.release();
     delete h;
     return 0;
 }
@@ -1993,18 +1998,29 @@ static int env_layers(const b200pf_handle *h, EnvLayers *l) {
     return 0;
 }
 
-// b200pf_env_step and b200pf_env_step_act: vec = 1 takes the step's action from the vector buffers of b200pf_act_bind
+// Where env_step takes the agent's action from: the sub_id / line_id pair (b200pf_env_step), the vector buffers of b200pf_act_bind
+// (b200pf_env_step_act), or the rows of the bound action table picked by one id per instance (b200pf_env_step_ids)
+enum ActMode { ACT_LEGACY = 0, ACT_VECTORS = 1, ACT_IDS = 2 };
+
 static int env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
-                    const int32_t *d_line_id, const int32_t *d_line_status, int vec, int from_reset, int is_dc, int max_iter,
-                    double tol_mva, int tight_cap, int stamp) {
+                    const int32_t *d_line_id, const int32_t *d_line_status, ActMode mode, const int32_t *d_action_id, int from_reset,
+                    int is_dc, int max_iter, double tol_mva, int tight_cap, int stamp) {
     if (!h) return fail(B200PF_E_ARG, "null handle");
     if (!env_bound(h)) return fail(B200PF_E_STATE, "environment not bound to the current series (b200pf_env_bind)");
     if ((!d_sub_id) != (!d_sub_bus) || (!d_line_id) != (!d_line_status)) return fail(B200PF_E_ARG, "ids without values");
     if (d_sub_id && (sub_bus_cols < h->env.max_sub || sub_bus_stride < sub_bus_cols)) return fail(B200PF_E_ARG, "sub_bus narrower than the largest substation");
-    if (vec && !layer_bound(h, h->act_batch)) return fail(B200PF_E_STATE, "no action buffers bound to the current environment (b200pf_act_bind)");
+    if (mode != ACT_LEGACY && !layer_bound(h, h->act_batch)) return fail(B200PF_E_STATE, "no action buffers bound to the current environment (b200pf_act_bind)");
+    if (mode == ACT_IDS && !h->n_act) return fail(B200PF_E_STATE, "no action table bound (b200pf_act_table_bind)");
+    if (mode == ACT_IDS && !d_action_id) return fail(B200PF_E_ARG, "null action ids");
     EnvLayers l;
     TRY(env_layers(h, &l));
-    l.act.vec = vec && !from_reset ? 1 : 0;
+    l.act.vec = mode != ACT_LEGACY && !from_reset ? 1 : 0;
+    ActIds ids{};
+    if (mode == ACT_IDS) {
+        l.act.set_bus = h->tab_set_bus; l.act.change_bus = h->tab_change_bus;
+        l.act.set_status = h->tab_set_status; l.act.change_status = h->tab_change_status;
+        if (!from_reset) { ids.id = d_action_id; ids.n = h->n_act; }
+    }
     CU(cudaSetDevice(h->device));
     const DevGrid &g = h->g;
     const int B = h->env_batch;
@@ -2017,10 +2033,10 @@ static int env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_s
     // 1. validation + apply (the apply kernel writes nothing when an input was rejected)
     CU(cudaMemsetAsync(a.ctl, 0, ENV_CTL_WORDS * 4, h->stream));
     if (a.sub_id || a.line_id || l.act.vec) {
-        pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a, l.act);
+        pf_kernel_env_validate<<<env_grid(B), 128, 0, h->stream>>>(a, l.act, ids);
         CU(cudaGetLastError());
     }
-    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.act);
+    pf_kernel_env_apply<<<env_grid(B), 128, 0, h->stream>>>(a, l.opp, h->opp_geo, h->opp_multi, l.act, ids);
     CU(cudaGetLastError());
     // 2. the step's one host wait: dirty count, bus cap, input error
     CU(cudaMemcpyAsync(h->h_env_ctl, a.ctl, ENV_CTL_WORDS * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -2028,7 +2044,8 @@ static int env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_s
     h->env_d2h += ENV_CTL_WORDS * 4; h->env_waits++;
     const int32_t *c = h->h_env_ctl;
     if (c[ENV_CTL_ERR])
-        return fail(B200PF_E_ARG, l.act.vec ? "vector action out of range (busbar outside [-1, n_busbar], -1 on an element other than a line end, "
+        return fail(B200PF_E_ARG, ids.id ? "action id outside [0, n) of the bound action table"
+                                : l.act.vec ? "vector action out of range (busbar outside [-1, n_busbar], -1 on an element other than a line end, "
                                               "change_bus without two busbars, line status outside {-1, 0, 1}, or a flag other than 0 / 1)"
                                             : "action out of range (substation / line id outside [-1, n), busbar outside [-1, n_busbar])");
     h->env_illegal += c[ENV_CTL_N_ILLEGAL];
@@ -2078,12 +2095,44 @@ static int env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_s
 extern "C" int b200pf_env_step(b200pf_handle *h, const int32_t *d_sub_id, const int8_t *d_sub_bus, int sub_bus_stride, int sub_bus_cols,
                                const int32_t *d_line_id, const int32_t *d_line_status, int from_reset, int is_dc, int max_iter,
                                double tol_mva, int tight_cap, int stamp) {
-    return env_step(h, d_sub_id, d_sub_bus, sub_bus_stride, sub_bus_cols, d_line_id, d_line_status, 0, from_reset, is_dc, max_iter, tol_mva,
-                    tight_cap, stamp);
+    return env_step(h, d_sub_id, d_sub_bus, sub_bus_stride, sub_bus_cols, d_line_id, d_line_status, ACT_LEGACY, nullptr, from_reset, is_dc,
+                    max_iter, tol_mva, tight_cap, stamp);
 }
 
 extern "C" int b200pf_env_step_act(b200pf_handle *h, int from_reset, int is_dc, int max_iter, double tol_mva, int tight_cap, int stamp) {
-    return env_step(h, nullptr, nullptr, 0, 0, nullptr, nullptr, 1, from_reset, is_dc, max_iter, tol_mva, tight_cap, stamp);
+    return env_step(h, nullptr, nullptr, 0, 0, nullptr, nullptr, ACT_VECTORS, nullptr, from_reset, is_dc, max_iter, tol_mva, tight_cap, stamp);
+}
+
+extern "C" int b200pf_env_step_ids(b200pf_handle *h, const int32_t *d_action_id, int from_reset, int is_dc, int max_iter, double tol_mva,
+                                   int tight_cap, int stamp) {
+    return env_step(h, nullptr, nullptr, 0, 0, nullptr, nullptr, ACT_IDS, d_action_id, from_reset, is_dc, max_iter, tol_mva, tight_cap, stamp);
+}
+
+extern "C" int b200pf_act_table_bind(b200pf_handle *h, const b200pf_act_table_desc *d) {
+    if (!h || !d) return fail(B200PF_E_ARG, "null pointer");
+    if (!layer_bound(h, h->act_batch)) return fail(B200PF_E_STATE, "no action rules bound to the current environment (b200pf_act_bind)");
+    if (d->n_act <= 0 || !d->set_bus || !d->change_bus || !d->set_status || !d->change_status) return fail(B200PF_E_ARG, "empty action table");
+    const HostGrid &hg = h->hg;
+    // every row under the rules of a vector action (act_input_ok, run here on the host), before anything is bound
+    std::vector<int32_t> line_of_pos(hg.dim_topo, -1);
+    for (int k = 0; k < hg.n_line; ++k) line_of_pos[hg.line_or_pos[k]] = k, line_of_pos[hg.line_ex_pos[k]] = k;
+    EnvArgs e{};
+    e.n_line = hg.n_line; e.dim_topo = hg.dim_topo; e.n_busbar = hg.n_busbar; e.line_of_pos = line_of_pos.data();
+    ActArgs r{};
+    r.set_bus = d->set_bus; r.change_bus = d->change_bus; r.set_status = d->set_status; r.change_status = d->change_status;
+    for (int i = 0; i < d->n_act; ++i)
+        if (!act_input_ok(e, r, i)) return fail(B200PF_E_ARG, "action table row " + std::to_string(i) + " out of range (busbar outside [-1, n_busbar], "
+                                                                "-1 on an element other than a line end, change_bus without two busbars, line status outside {-1, 0, 1}, or a flag other than 0 / 1)");
+    TRY(unbind(h, &h->n_act, h->act_table_bufs));
+    const size_t n = (size_t)d->n_act, nt = (size_t)hg.dim_topo, nl = (size_t)hg.n_line;
+    DevBufs &o = h->act_table_bufs;
+    TRY(dev_alloc(h, o, h->tab_set_bus, n * nt, d->set_bus));
+    TRY(dev_alloc(h, o, h->tab_change_bus, n * nt, d->change_bus));
+    TRY(dev_alloc(h, o, h->tab_set_status, n * nl, d->set_status));
+    TRY(dev_alloc(h, o, h->tab_change_status, n * nl, d->change_status));
+    CU(cudaStreamSynchronize(h->stream));
+    h->n_act = d->n_act;
+    return 0;
 }
 
 extern "C" int b200pf_act_bind(b200pf_handle *h, const b200pf_act_desc *d) {

@@ -98,6 +98,16 @@ struct ActArgs {
     uint8_t *aff_sub;                               // [batch][n_sub] library scratch: substations the legal vector action touched
 };
 
+// The discrete action ids of a b200pf_env_step_ids step: ActArgs' four pointers are then the n rows of the bound action table
+// (b200pf_act_table_bind) and instance i acts with row id[i].
+struct ActIds {
+    const int32_t *id;                              // [batch]
+    int n;                                          // rows of the table
+};
+
+// the row of the four vectors instance i acts with (ids: NULL without an action table)
+ENV_HD inline size_t act_row(const ActIds *ids, int i) { return ids ? (size_t)ids->id[i] : (size_t)i; }
+
 #if defined(__CUDA_ARCH__)
 #define ENV_ATOMIC_ADD(p, v) atomicAdd((p), (v))
 #define ENV_ATOMIC_MAX(p, v) atomicMax((p), (v))
@@ -127,8 +137,10 @@ ENV_HD inline bool env_input_ok(const EnvArgs &a, int i) {
 }
 
 // The vector action of instance i: busbars in [-1, n_busbar] with -1 on line ends only (detaching a load, generator or storage unit
-// is not restated), change_bus only with two busbars per substation, line statuses in {-1, 0, 1}.
-ENV_HD inline bool act_input_ok(const EnvArgs &a, const ActArgs &r, int i) {
+// is not restated), change_bus only with two busbars per substation, line statuses in {-1, 0, 1}.  With an action table (ids), its
+// id in [0, n): the table's rows were checked when it was bound.
+ENV_HD inline bool act_input_ok(const EnvArgs &a, const ActArgs &r, int i, const ActIds *ids = nullptr) {
+    if (ids) return ids->id[i] >= 0 && ids->id[i] < ids->n;
     const int8_t *sb = r.set_bus + (size_t)i * a.dim_topo;
     const uint8_t *cb = r.change_bus + (size_t)i * a.dim_topo;
     for (int p = 0; p < a.dim_topo; ++p) {
@@ -188,14 +200,15 @@ ENV_HD inline int act_topo_value(int v, uint8_t change, int8_t set) {
 // status the previous step left, legality, and _BackendAction.__iadd__'s application (line status change then set, change_bus then
 // set_bus, then the reconciliation of disconnected / reconnected line ends).  A disconnected end is one <= 0.  Writes is_ambiguous,
 // is_illegal, the impacted lines (affl) and substations (aff_sub) of a legal action; -> the topology may have changed.
-ENV_HD inline bool act_vec_instance(const EnvArgs &a, const ActArgs &r, int i, bool done, uint8_t *affl) {
+ENV_HD inline bool act_vec_instance(const EnvArgs &a, const ActArgs &r, int i, bool done, uint8_t *affl, const ActIds *ids = nullptr) {
     const int nl = a.n_line, ns = a.n_sub, nt = a.dim_topo;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * nt;
-    const int8_t *sb = r.set_bus + (size_t)i * nt;
-    const uint8_t *cb = r.change_bus + (size_t)i * nt;
-    const int8_t *ss = r.set_status + (size_t)i * nl;
-    const uint8_t *cs = r.change_status + (size_t)i * nl;
+    const size_t row = act_row(ids, i);
+    const int8_t *sb = r.set_bus + row * nt;
+    const uint8_t *cb = r.change_bus + row * nt;
+    const int8_t *ss = r.set_status + row * nl;
+    const uint8_t *cs = r.change_status + row * nl;
     uint8_t *affs = r.aff_sub + (size_t)i * ns;
     for (int s = 0; s < ns; ++s) affs[s] = 0;
     // 1. BaseAction._check_for_ambiguity, topology part (baseAction.py:3558-3565, :3670-3771)
@@ -304,9 +317,9 @@ ENV_HD inline int env_count_buses(const EnvArgs &a, const int8_t *tv) {
 
 // BatchedEnv._apply_agent (or _apply_actions, ac->vec) followed by _apply_environment and the opponent's attack (o: NULL or no
 // opponent bound), for instance i (g: the GeometricOpponent's part, m: the GeometricOpponentMultiArea's; NULL for the other kinds;
-// ac: NULL or the bound action rules)
+// ac: NULL or the bound action rules; ids: NULL or the ids into the action table of a b200pf_env_step_ids step)
 ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o = nullptr, const OppGeoArgs *g = nullptr,
-                                      const OppMultiArgs *m = nullptr, const ActArgs *ac = nullptr) {
+                                      const OppMultiArgs *m = nullptr, const ActArgs *ac = nullptr, const ActIds *ids = nullptr) {
     const int nl = a.n_line;
     int8_t *tv = a.topo + (size_t)i * a.n_topo_in;
     int8_t *lb = a.last_bus + (size_t)i * a.dim_topo;
@@ -324,7 +337,7 @@ ENV_HD inline void env_apply_instance(const EnvArgs &a, int i, const OppArgs *o 
     }
     if (ac && ac->is_ambiguous && (a.from_reset || !ac->vec)) ac->is_ambiguous[i] = 0;
     if (!a.from_reset && ac && ac->vec) {
-        dirty = act_vec_instance(a, *ac, i, done, affl);
+        dirty = act_vec_instance(a, *ac, i, done, affl, ids);
     } else if (!a.from_reset) {
         bool has_sub = false, has_line = false;
         int sid = -1, lid = -1, lst = 0;
@@ -581,18 +594,18 @@ ENV_HD inline void env_observed_instance(const EnvArgs &a, int i) {
 }
 
 #if defined(__CUDACC__)
-// (r.aff_sub is NULL when no action rules are bound)
-__global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a, ActArgs r) {
+// (r.aff_sub is NULL when no action rules are bound; ids.id NULL without an action table)
+__global__ void __launch_bounds__(128) pf_kernel_env_validate(EnvArgs a, ActArgs r, ActIds ids) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < a.batch && !(r.vec ? act_input_ok(a, r, i) : env_input_ok(a, i))) atomicOr(&a.ctl[ENV_CTL_ERR], 1);
+    if (i < a.batch && !(r.vec ? act_input_ok(a, r, i, ids.id ? &ids : nullptr) : env_input_ok(a, i))) atomicOr(&a.ctl[ENV_CTL_ERR], 1);
 }
 
 // one thread per instance; nothing is written when the validation flagged an input
-__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, ActArgs r) {
+__global__ void __launch_bounds__(128) pf_kernel_env_apply(EnvArgs a, OppArgs o, OppGeoArgs g, OppMultiArgs m, ActArgs r, ActIds ids) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.batch || *(volatile int32_t *)&a.ctl[ENV_CTL_ERR]) return;
     env_apply_instance(a, i, &o, o.kind == OPP_GEOMETRIC ? &g : nullptr, o.kind == OPP_GEOMETRIC_MULTI ? &m : nullptr,
-                       r.aff_sub ? &r : nullptr);
+                       r.aff_sub ? &r : nullptr, ids.id ? &ids : nullptr);
 }
 
 __global__ void __launch_bounds__(128) pf_kernel_env_post(EnvArgs a, AlertArgs al, AlarmArgs am, ActArgs r) {

@@ -47,6 +47,7 @@ ABI_SYMBOLS = (
     "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state",
     "b200pf_alert_bind", "b200pf_alert_get_state", "b200pf_alert_set_state",
     "b200pf_alarm_bind", "b200pf_alarm_get_state", "b200pf_alarm_set_state", "b200pf_act_bind", "b200pf_env_step_act",
+    "b200pf_act_table_bind", "b200pf_env_step_ids",
 )
 
 
@@ -142,6 +143,12 @@ class ActDesc(C.Structure):
         ("line_area", C.c_void_p), ("set_bus", C.c_void_p), ("change_bus", C.c_void_p), ("set_status", C.c_void_p),
         ("change_status", C.c_void_p), ("is_ambiguous", C.c_void_p),
     ]
+
+
+class ActTableDesc(C.Structure):
+    """``b200pf_act_table_desc`` of include/b200pf.h"""
+    _fields_ = [("n_act", C.c_int32), ("set_bus", C.c_void_p), ("change_bus", C.c_void_p), ("set_status", C.c_void_p),
+                ("change_status", C.c_void_p)]
 
 
 class AlertDesc(C.Structure):
@@ -329,12 +336,14 @@ def load_library():
     lib.b200pf_alarm_set_state.argtypes = [vp] + [vp] * 10
     lib.b200pf_act_bind.argtypes = [vp, C.POINTER(ActDesc)]
     lib.b200pf_env_step_act.argtypes = [vp, i32, i32, i32, f64, i32, i32]
+    lib.b200pf_act_table_bind.argtypes = [vp, C.POINTER(ActTableDesc)]
+    lib.b200pf_env_step_ids.argtypes = [vp, vp, i32, i32, i32, f64, i32, i32]
     for nm in ("b200pf_env_bind", "b200pf_env_step", "b200pf_env_reset", "b200pf_env_get_state", "b200pf_env_set_state",
                "b200pf_env_pointers", "b200pf_observe_device", "b200pf_env_stats", "b200pf_opp_bind", "b200pf_opp_get_state",
                "b200pf_opp_set_state", "b200pf_opp_geo_bind", "b200pf_opp_geo_get_state", "b200pf_opp_geo_set_state",
                "b200pf_opp_multi_bind", "b200pf_opp_multi_get_state", "b200pf_opp_multi_set_state", "b200pf_alert_bind",
                "b200pf_alert_get_state", "b200pf_alert_set_state", "b200pf_alarm_bind", "b200pf_alarm_get_state",
-               "b200pf_alarm_set_state", "b200pf_act_bind", "b200pf_env_step_act"):
+               "b200pf_alarm_set_state", "b200pf_act_bind", "b200pf_env_step_act", "b200pf_act_table_bind", "b200pf_env_step_ids"):
         getattr(lib, nm).restype = i32
     lib.b200pf_redo_launch_count.argtypes = [vp]
     lib.b200pf_redo_launch_count.restype = C.c_int64
@@ -774,6 +783,22 @@ class PowerFlowEngine:
         """:meth:`env_step` with the action taken from the vector buffers :meth:`act_bind` bound (``b200pf_env_step_act``)"""
         self._check(self.lib.b200pf_env_step_act(self.h, int(bool(from_reset)), int(bool(is_dc)), int(max_iter), float(tol_mva),
                                                  int(bool(tight_cap)), int(stamp)), "b200pf_env_step_act")
+
+    def env_step_ids(self, d_action_id: int, from_reset: bool = False, is_dc: bool = False, max_iter: int = 10, tol_mva: float = 1e-8,
+                     tight_cap: bool = True, stamp: int = 0):
+        """:meth:`env_step_act` with instance i acting with row ``d_action_id[i]`` (device int32 [B]) of the table
+        :meth:`act_table_bind` bound (``b200pf_env_step_ids``)"""
+        self._check(self.lib.b200pf_env_step_ids(self.h, C.c_void_p(int(d_action_id)), int(bool(from_reset)), int(bool(is_dc)), int(max_iter),
+                                                 float(tol_mva), int(bool(tight_cap)), int(stamp)), "b200pf_env_step_ids")
+
+    def act_table_bind(self, set_bus, change_bus, set_line_status, change_line_status):
+        """the discrete action table (``b200pf_act_table_bind``): host arrays int8 / bool [n, dim_topo] and int8 / bool [n, n_line],
+        checked row by row and copied to device memory the library owns"""
+        sb, ss = np.ascontiguousarray(set_bus, np.int8), np.ascontiguousarray(set_line_status, np.int8)
+        cb, cs = np.ascontiguousarray(change_bus, np.uint8), np.ascontiguousarray(change_line_status, np.uint8)
+        d = ActTableDesc(n_act=len(sb), set_bus=sb.ctypes.data, change_bus=cb.ctypes.data, set_status=ss.ctypes.data,
+                         change_status=cs.ctypes.data)
+        self._check(self.lib.b200pf_act_table_bind(self.h, C.byref(d)), "b200pf_act_table_bind")
 
     def act_bind(self, max_sub_changed: int, max_line_status_changed: int, n_area: int, sub_area, line_area, d_set_bus: int,
                  d_change_bus: int, d_set_status: int, d_change_status: int, d_is_ambiguous: int):

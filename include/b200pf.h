@@ -427,6 +427,25 @@ typedef struct b200pf_act_desc {
 int b200pf_act_bind(b200pf_handle *h, const b200pf_act_desc *desc);
 int b200pf_env_step_act(b200pf_handle *h, int from_reset, int is_dc, int max_iter, double tol_mva, int tight_cap, int stamp);
 
+/* A discrete action table for the device environment: n_act rows of grid2op's native topology action (IdToAct's list, say), each
+ * instance acting with one row picked by its id.  b200pf_act_table_bind needs b200pf_act_bind (the rules, is_ambiguous and the
+ * library's scratch come from there).  It checks every row with the rules of b200pf_env_step_act's vectors and fails with
+ * B200PF_E_ARG, binding nothing, when one is out of range; else it copies the four HOST arrays (the layout of b200pf_act_desc's
+ * buffers with n_act rows instead of batch) to device memory the library owns.  A new bind replaces the table.
+ * b200pf_env_step_ids is b200pf_env_step_act with instance i taking row d_action_id[i] (DEVICE int32 [batch]) of the table.  An id
+ * outside [0, n_act) fails the call with B200PF_E_ARG before anything is written.  Launches, host waits and bytes moved per step
+ * are those of b200pf_env_step_act; no action data is copied. */
+typedef struct b200pf_act_table_desc {
+    int32_t n_act;                      /* rows */
+    const int8_t *set_bus;              /* [n_act][dim_topo] */
+    const uint8_t *change_bus;          /* [n_act][dim_topo] */
+    const int8_t *set_status;           /* [n_act][n_line] */
+    const uint8_t *change_status;       /* [n_act][n_line] */
+} b200pf_act_table_desc;
+int b200pf_act_table_bind(b200pf_handle *h, const b200pf_act_table_desc *desc);
+int b200pf_env_step_ids(b200pf_handle *h, const int32_t *d_action_id, int from_reset, int is_dc, int max_iter, double tol_mva, int tight_cap,
+                        int stamp);
+
 /* Line-attack opponent of the device environment (csrc/b200pf_opp.cuh): grid2op's OpponentSpace with BaseActionBudget and a
  * RandomLineOpponent (kind 1) or a WeightedRandomOpponent (kind 2), attacking one line at a time with set_line_status -1, each
  * instance with its own numpy-legacy random stream (RandomState: MT19937 state of 624 words and a position, as get_state() gives

@@ -9,7 +9,12 @@ one-substation / one-line actions through the legacy arguments and through the s
 environments alternating, to isolate the cost of the wider input; (2) l2rpn_idf_2023 at batch 1024 with its RulesByArea:
 multi-substation set_bus / change_bus actions with a few line statuses.
 
-    python scripts/bench_env_tensor.py [--steps 50] [--warmup 5] [--repeats 5] [--vector]
+``--ids``: discrete action ids into an ``ActionTable`` on the tensor path, ids drawn on the GPU.  (1) case14 at batch 4096, protections
+off, the unitary table (IdToAct's 487 topology actions): the same actions as ids and as the four vectors gathered with torch from
+the table, the two environments alternating, to isolate what the id encoding saves against the vector encoding; (2) l2rpn_idf_2023
+at batch 1024 with its RulesByArea and the full unitary table (147,260 rows, 214 MB): the cost of row reads scattered over it.
+
+    python scripts/bench_env_tensor.py [--steps 50] [--warmup 5] [--repeats 5] [--vector | --ids]
 """
 import argparse
 import os
@@ -157,7 +162,8 @@ def draw_multi(env, gen, dev):
 
 
 def run_vector(name, B, steps, warmup, repeats, modes, rules_by_area=None):
-    """``modes``: ("legacy", "vector") for the same one-substation actions in the two encodings, or ("multi",)"""
+    """``modes``: ("legacy", "vector") for the same one-substation actions in the two encodings, ("multi",), or ("ids", "rows")
+    / ("ids",) for ids into the unitary action table and the same rows as vectors"""
     import torch
     from conftest import env_grid
     from grid2op_b200.batched_env import BatchedEnv
@@ -169,11 +175,20 @@ def run_vector(name, B, steps, warmup, repeats, modes, rules_by_area=None):
     folders = list_scenarios(os.path.join(env_dir, "chronics"))[:4]
     chron = load_scenarios(os.path.join(env_dir, "chronics"), gm, scenarios=folders)
     dev = torch.device("cuda", 0)
+    table = tab = None
+    if "ids" in modes or "rows" in modes:
+        from grid2op_b200.action_table import ActionTable
+        table = ActionTable.unitary(gm)
+        tab = [torch.as_tensor(np.array(x), device=dev) for x in (table.set_bus, table.change_bus, table.set_line_status,
+                                                                     table.change_line_status)]
+        print(f"{name}: action table of {table.n} rows, {sum(x.numel() for x in tab) / 1e6:.1f} MB")
     envs, gens = {}, {}
     for mode in modes:
         e = BatchedEnv(gm, chron, B, nb_timestep_cooldown_line=2, nb_timestep_cooldown_sub=2, protections=False,
                        rules_by_area=rules_by_area, max_sub_changed=1 if rules_by_area else 3, max_line_status_changed=1 if rules_by_area else 2)
         e.enable_observation(env_dir, scenarios=folders)
+        if mode == "ids":
+            e.set_action_table(table)
         envs[mode] = e
         gens[mode] = torch.Generator(device=dev)
         gens[mode].manual_seed(0)
@@ -183,6 +198,13 @@ def run_vector(name, B, steps, warmup, repeats, modes, rules_by_area=None):
         if mode == "multi":
             sb, cb, ss = draw_multi(e, gens[mode], dev)
             _, done, _ = e.step_tensors(set_bus=sb, change_bus=cb, set_line_status=ss)
+        elif mode in ("ids", "rows"):
+            ids = torch.randint(0, table.n, (B,), generator=gens[mode], device=dev, dtype=torch.int32)
+            if mode == "ids":
+                _, done, _ = e.step_tensors(action_id=ids)
+            else:
+                _, done, _ = e.step_tensors(set_bus=tab[0][ids], change_bus=tab[1][ids], set_line_status=tab[2][ids],
+                                            change_line_status=tab[3][ids])
         else:
             sub, bus, line, lst = draw(e, gens[mode], dev)
             if mode == "legacy":
@@ -227,8 +249,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--vector", action="store_true")
+    ap.add_argument("--ids", action="store_true")
     args = ap.parse_args()
     print("card, power limit:", card())
+    if args.ids:
+        from test_env_actions_gpu import _idf_rule_areas
+        run_vector("l2rpn_case14_sandbox", 4096, args.steps, args.warmup, args.repeats, ("ids", "rows"))
+        run_vector("l2rpn_idf_2023", 1024, args.steps, args.warmup, args.repeats, ("ids",), rules_by_area=_idf_rule_areas())
+        return
     if args.vector:
         from test_env_actions_gpu import _idf_rule_areas
         run_vector("l2rpn_case14_sandbox", 4096, args.steps, args.warmup, args.repeats, ("legacy", "vector"))
